@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """Benchmark of the `inference` hot path (BASELINE.json metric: Mvoxels/s for the 3-channel
-affinity U-Net on a 1024^3 uint8 chunk at 1/2/4/8 B200).
+affinity U-Net on a 1024^3 uint8 chunk per H100).
 
     python bench.py --gpus N --steps K --warmup W          # this repo's CUDA path
     python bench.py --impl reference --gpus N ...           # the reference algorithm on the host CPUs
+    python bench.py ... --dump-outputs DIR                  # also write what the last timed step computed (DIR/*.npy)
 
 A "step" is one pass of the hot path over one synthetic chunk per GPU (weak scaling: one
 independent chunk per rank, no data-path collective).  Prints ONE JSON line (rank 0).
@@ -58,7 +59,7 @@ def synthetic_chunk(shape, seed, pinned=True):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -263,6 +264,15 @@ def split_chunk_block(inf, Chunk, patch, overlap, rank, world, local_rank, args,
             "max_abs_vs_single_gpu": max_abs, "tolerance": 2e-6}
 
 
+def dump_outputs(path, d_out):
+    """The affinity map of the last timed step, (channels, z, y, x) float32: every 16th plane, every 4th row and column
+    (at most 64 MB for the 1024^3 workload; the whole map when it is that small)."""
+    os.makedirs(path, exist_ok=True)
+    step = (1, 16, 4, 4) if d_out.numel() * 4 > (64 << 20) else (1, 1, 1, 1)
+    sample = d_out[::step[0], ::step[1], ::step[2], ::step[3]].float().cpu().numpy()
+    np.save(os.path.join(path, "affinity_sample.npy"), np.ascontiguousarray(sample, dtype=np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -279,6 +289,8 @@ def main():
     ap.add_argument("--no-alt-precision", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the affinity map of the last timed step "
+                    "(a fixed strided sample of it, float32) to DIR/affinity_sample.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", 0))
@@ -291,7 +303,7 @@ def main():
     config = {"workload": f"{'x'.join(map(str, chunk_shape))} uint8 chunk per GPU, 3-ch affinity UNet3L(16,32,64), "
                           f"patch {'x'.join(map(str, patch))} overlap {'x'.join(map(str, overlap))}, mask_output_chunk",
               "patches_per_chunk": P, "batch_size": args.batch_size, "chunks": world,
-              "l2_policy": "inputs and outputs (1 GB + 12.9 GB per step) are far larger than the 126 MB L2",
+              "l2_policy": "inputs and outputs (1 GB + 12.9 GB per step) are far larger than the 50 MB L2",
               "parallelism": f"{world} independent chunk(s), one per GPU, no collective"}
 
     if args.impl == "reference":
@@ -374,6 +386,8 @@ def main():
         torch.cuda.cudart().cudaProfilerStop()
     barrier()
     ms = max_over_ranks(e0.elapsed_time(e1))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, d_out)
     clocks = sampler.stop() if sampler else None
     launches = eng.last_timing()["launches"]
     value = nvox * world * args.steps / (ms / 1e3) / 1e6
@@ -393,36 +407,24 @@ def main():
     conv_launches = sum(layers[k][1] for k in CONV3_FLOP if k in layers)
     pvox = int(np.prod(patch))
     conv_flop = sum(v for k, v in CONV3_FLOP.items() if k in layers) * P * pvox
-    tf_peak = peaks.get("bf16_tflops_sustained", 1400.0)
+    tf_peak = peaks.get("bf16_tflops_sustained", 989.0)   # H100 SXM data sheet, dense FP16/BF16
     # dominant kernel = the 3x3x3 layer with the largest share of the step (dec0.0 / dec1.0, the concat layers)
     dom = max((k for k in CONV3_FLOP if k in layers), key=lambda k: layers[k][0])
     dom_ms, dom_launches = layers[dom]
     dom_flop_per_launch = CONV3_FLOP[dom] * P * pvox / dom_launches
     achieved = dom_flop_per_launch / (dom_ms / dom_launches / 1e3) / 1e12 if dom_ms > 0 else 0.0
     traffic, pipe_note = None, ""
-    try:  # DRAM bytes per launch from the committed ncu --set full capture (profiles/r01_ncu_traffic.json), scaled to this batch
-        prof = "r02_ncu_traffic.json" if eng.params.precision == 3 else "r01_ncu_traffic.json"   # --set full capture of the same precision mode
-        tl = json.load(open(os.path.join(ROOT, "profiles", prof)))["layers"]
-        t = tl.get(dom)
-        if t and t.get("dram_bytes_per_patch"):
-            traffic = t["dram_bytes_per_patch"] * P / dom_launches
-        pipes = [v["tensor_pipe_active_pct"] for k, v in tl.items() if k in CONV3_FLOP and "conv3" in v.get("kernel", "")]
-        if pipes:
-            pipe_note = "; ncu tensor-pipe active %.0f-%.0f %% over the 3x3x3 layers, %.0f %% on this one" % (
-                min(pipes), max(pipes), (t or {}).get("tensor_pipe_active_pct", float("nan")))
-    except Exception:
-        pass
-    roofline = {"bound": "tensor", "kernel": f"{dom}: tcgen05 3x3x3 convolution (conv3_ts_umma_kernel: z-stacked, A operand in tensor memory)",
+    roofline = {"bound": "tensor", "kernel": f"{dom}: wgmma 3x3x3 convolution (conv3_wgmma_kernel)",
                 "achieved": achieved, "peak": tf_peak, "unit": "TFLOP/s", "frac": achieved / tf_peak,
-                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback (B200_PROFILING.md)",
+                "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "H100 SXM data sheet (not reached)",
                 "traffic": traffic, "launches": dom_launches, "ms_per_launch": dom_ms / max(dom_launches, 1),
                 "algorithmic_flop_per_launch": dom_flop_per_launch,
                 "note": ("the f16f8 mode executes 2x these algorithmic FLOPs on the tensor pipe (one fp16 + one e4m3 K=32 product per multiply)"
                          if eng.params.precision == 3 else "the fp16 hi/lo split (f16x3) executes 3x these algorithmic FLOPs on the tensor pipe") + pipe_note +
-                        " (profiles/r02_ncu_full_summary.md / r01_ncu_full_summary.md)",
+                        "",
                 "conv_stack": {"achieved": conv_flop / (conv_ms / 1e3) / 1e12 if conv_ms > 0 else 0.0, "unit": "TFLOP/s",
                                "ms_per_chunk": conv_ms, "launches": conv_launches, "algorithmic_flop_per_chunk": conv_flop}}
-    hbm_peak = peaks.get("hbm_gbs", 6650.0)
+    hbm_peak = peaks.get("hbm_gbs", 3350.0)   # H100 SXM data sheet
     pv = P * int(np.prod(patch))
     mem = {}
     parts = {0: 0, 1: 2, 2: 1, 3: 2}[eng.params.precision]
@@ -550,9 +552,9 @@ def main():
         split = split_chunk_block(inf, Chunk, patch, overlap, rank, world, local_rank, args, barrier, max_over_ranks)
 
     if rank == 0:
-        precision = {0: "f32 (FFMA, CUDA cores)", 1: "f16x3 hi/lo split on tcgen05, f32 accumulate",
-                     2: "f16 on tcgen05, f32 accumulate",
-                     3: "f16f8: fp16 main product + one e4m3 (K=32) product carrying both hi/lo correction terms on tcgen05, f32 accumulate"}[eng.params.precision]
+        precision = {0: "f32 (FFMA, CUDA cores)", 1: "f16x3 hi/lo split on wgmma, f32 accumulate",
+                     2: "f16 on wgmma, f32 accumulate",
+                     3: "f16f8: fp16 main product + one e4m3 (K=32) product carrying both hi/lo correction terms on wgmma, f32 accumulate"}[eng.params.precision]
         print(json.dumps({
             "metric": "Mvoxels/s", "value": value, "unit": "Mvoxels/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak",

@@ -1,7 +1,7 @@
-"""chunkflow_b200 -- B200-native implementation of chunkflow's ``inference`` hot path.
+"""chunkflow_b200 -- H100-native implementation of chunkflow's ``inference`` hot path.
 
 Host side in Python (mirrors the reference's operator / plugin interface), hot path as
-hand-written sm_100a CUDA kernels behind a C-ABI shared library
+hand-written sm_90a CUDA kernels behind a C-ABI shared library
 (``include/chunkflow_b200.h``, loaded with ctypes by :mod:`chunkflow_b200._native`).
 """
 from .chunk import Chunk  # noqa: F401

@@ -7,8 +7,8 @@ expose ``load_model(weight_path)`` or ``InstantiatedModel`` (plus optional
 contract, so the SAME file drives
 
 * the reference's own ``-f pytorch`` CPU path (the parity oracle), and
-* the B200 path, which reads :data:`LAYER_SPEC` / the ``state_dict`` and packs the
-  weights into the device layout of the hand-written sm_100a kernels.
+* the device path, which reads :data:`LAYER_SPEC` / the ``state_dict`` and packs the
+  weights into the device layout of the hand-written sm_90a kernels.
 
 It must stay self-contained (no package-relative imports): the reference executes it
 through ``SourceFileLoader("Model", fname)`` (``chunkflow/lib/__init__.py:5-16``).

@@ -1,9 +1,9 @@
-// "f16f8" activation / weight number format of the tcgen05 convolution stack (precision mode CFB_PRECISION_F16F8_UMMA).
+// "f16f8" activation / weight number format of the wgmma convolution stack (precision mode CFB_PRECISION_F16F8_UMMA).
 //
 // The f16x3 mode spends THREE tensor-core products per multiply (a_hi w_hi + a_hi w_lo + a_lo w_hi, all fp16).  The two
 // correction terms are 2^-11 of the main one, so they need only a few significant bits themselves: here they run as ONE
 // fp8 (e4m3) product of twice the K depth -- kind::f8f6f4, K = 32 = [a | a_lo] x [w_lo ; w] -- at the price of one fp16
-// MMA, i.e. TWO tensor-core products per multiply instead of three, accumulating in the same fp32 TMEM columns:
+// MMA, i.e. TWO tensor-core products per multiply instead of three, accumulating in the same fp32 accumulators:
 //
 //     acc  =  H * WH            (kind::f16,    K = 16 channels)
 //          +  A8 * WL8 + L8 * W8 (kind::f8f6f4, K = 32 = 16 channels x {A8, L8})
@@ -19,10 +19,10 @@
 //                                                           fp16-level corrections -- up to 2047, clamped beyond)
 //     beta  = 2^14 / wmax', delta = beta / 64              (per layer, wmax' = max |w| rounded up to a power of two)
 // The epilogue multiplies the accumulator by 1 / (alpha * beta).  Error of one product: the dropped a_lo w_lo (2^-24) plus
-// the e4m3 rounding (2^-4 relative) of two terms that are 2^-12 of the product: ~2^-16 worst case, ~2^-17.5 rms --
-// measured max-abs error of the whole network against the fp32 reference in DESIGN.md.
+// the e4m3 rounding (2^-4 relative) of two terms that are 2^-12 of the product: ~2^-16 worst case, ~2^-17.5 rms; the
+// tests assert the whole network within 5e-4 max-abs of the fp32 reference.
 //
-// HBM layout ("CP8", kernels_umma.cuh) is unchanged: planes of 16-byte voxel records, plane = chunk * 2 + part for
+// HBM layout ("CP8", kernels_conv.cuh) is unchanged: planes of 16-byte voxel records, plane = chunk * 2 + part for
 // 8-channel chunk `chunk`.  Per K step (two chunks c0 = 2k, c1 = 2k + 1, i.e. channels 16k .. 16k + 15):
 //     (c0, part 0) = H  channels 0..7      (c1, part 0) = H  channels 8..15      (fp16 x 8)
 //     (c0, part 1) = A8 channels 0..15     (c1, part 1) = L8 channels 0..15      (e4m3 x 16)

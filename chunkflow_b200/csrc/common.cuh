@@ -1,4 +1,4 @@
-// Shared declarations of the chunkflow_b200 native library (sm_100a only).
+// Shared declarations of the chunkflow_b200 native library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

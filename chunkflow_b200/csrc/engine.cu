@@ -450,8 +450,8 @@ int cfb_create(const cfb_params* params, cfb_handle* out) {
     cudaDeviceProp prop;
     CFB_CUDA(cudaGetDeviceProperties(&prop, p.device));
     e->device_name = prop.name;
-    if (prop.major != 10) {
-      set_last_error(std::string("chunkflow_b200 kernels are built for sm_100a only; device is ") + prop.name);
+    if (prop.major != 9 || prop.minor != 0) {
+      set_last_error(std::string("chunkflow_b200 kernels are built for sm_90a (H100) only; device is ") + prop.name);
       return CFB_ERR_CUDA;
     }
     e->h_mask = build_patch_mask(e->op, e->ovl);

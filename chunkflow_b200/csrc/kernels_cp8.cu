@@ -1,7 +1,7 @@
 // CUDA-core kernels on the CP8 (chunk-planar fp16, optional hi/lo split) activation layout:
 // layout conversion, the first (Cin = 1) convolution fused with patch extraction, max pooling,
-// transposed convolution and the 1x1x1 head.  See kernels_umma.cuh.
-#include "kernels_umma.cuh"
+// transposed convolution and the 1x1x1 head.  See kernels_conv.cuh.
+#include "kernels_conv.cuh"
 
 #include "act_format.cuh"
 #include "chunkflow_b200.h"
@@ -360,7 +360,7 @@ head_blend_cp8_kernel(const uint4* __restrict__ in, const float* __restrict__ w,
 int grid_for(size_t items) {
   size_t b = (items + kT - 1) / kT;
   if (b < 1) b = 1;
-  if (b > 148 * 16) b = 148 * 16;
+  if (b > 132 * 16) b = 132 * 16;
   return (int)b;
 }
 

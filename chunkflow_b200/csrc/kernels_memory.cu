@@ -1,4 +1,4 @@
-// HBM-bound kernels of the inference hot path (sm_100a).  See kernels_memory.cuh.
+// HBM-bound kernels of the inference hot path (sm_90a).  See kernels_memory.cuh.
 #include "kernels_memory.cuh"
 
 #include <algorithm>
@@ -293,7 +293,7 @@ any_nonzero_kernel(const T* __restrict__ p, int64_t n, unsigned int* __restrict_
   if (__any_sync(0xffffffffu, nz) && (threadIdx.x & 31) == 0) atomicOr(flag, 1u);
 }
 
-int grid_for(int64_t items, int max_blocks = 148 * 16) {
+int grid_for(int64_t items, int max_blocks = 132 * 16) {
   int64_t b = ceil_div64(items, kThreads);
   if (b < 1) b = 1;
   if (b > max_blocks) b = max_blocks;
@@ -372,7 +372,7 @@ __global__ void __launch_bounds__(256) halo_add_kernel(float* __restrict__ dst, 
 
 void launch_halo_add(float* dst, const float* src, int64_t n, cudaStream_t s) {
   if (n <= 0) return;
-  int64_t blocks = std::min<int64_t>(ceil_div64(n / 4 + 1, 256), 148 * 16);
+  int64_t blocks = std::min<int64_t>(ceil_div64(n / 4 + 1, 256), 132 * 16);
   halo_add_kernel<<<(int)blocks, 256, 0, s>>>(dst, src, n);
   CFB_LAUNCH_CHECK();
 }

@@ -1,4 +1,4 @@
-// fp32 CUDA-core network kernels (sm_100a).  See kernels_simt.cuh.
+// fp32 CUDA-core network kernels (sm_90a).  See kernels_simt.cuh.
 #include "kernels_simt.cuh"
 
 namespace cfb {
@@ -174,7 +174,7 @@ head_sigmoid_f32_kernel(const float* __restrict__ in, const float* __restrict__ 
 int grid_for(int64_t items) {
   int64_t b = ceil_div64(items, 256);
   if (b < 1) b = 1;
-  if (b > 148 * 16) b = 148 * 16;
+  if (b > 132 * 16) b = 132 * 16;
   return (int)b;
 }
 

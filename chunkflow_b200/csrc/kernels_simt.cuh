@@ -1,5 +1,5 @@
 // fp32 CUDA-core (FFMA) network kernels: the exact-fp32 precision mode and the device-side
-// cross-check for the tcgen05 kernels.  Activations are planar (batch, C, Z, Y, X) fp32.
+// cross-check for the wgmma kernels.  Activations are planar (batch, C, Z, Y, X) fp32.
 #pragma once
 #include "common.cuh"
 

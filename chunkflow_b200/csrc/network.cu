@@ -111,17 +111,13 @@ bool Network::load(const std::map<std::string, std::vector<float>>& host_w, int 
     CFB_CUDA(cudaMemcpy(L.bias, bi->second.data(), bi->second.size() * sizeof(float), cudaMemcpyHostToDevice));
     if (umma() && sp.taps == 27 && sp.cin >= 16)
       pack_conv3_weights(wi->second.data(), bi->second.data(), sp.cin, cout, fmt(), L.packed);
-    if (umma() && sp.taps == 27 && sp.cin == 1) {
-      pack_first_conv_weights(wi->second.data(), bi->second.data(), fmt(), L.packed);
-      if (cout == 16) pack_first_conv_ts_weights(wi->second.data(), L.packed);
-      if (cout == 16) {
-        for (int t = 0; t < 27; ++t)
-          for (int c = 0; c < 16; ++c) first_w_.w[t][c] = wi->second[(size_t)c * 27 + t];
-        for (int c = 0; c < 16; ++c) first_w_.b[c] = bi->second[c];
-      }
-    }
     if (umma() && sp.taps == 4)
       pack_convT_weights(wi->second.data(), bi->second.data(), sp.cin, cout, fmt(), L.packed);
+    if (umma() && sp.taps == 27 && sp.cin == 1 && cout == 16) {
+      for (int t = 0; t < 27; ++t)
+        for (int c = 0; c < 16; ++c) first_w_.w[t][c] = wi->second[(size_t)c * 27 + t];
+      for (int c = 0; c < 16; ++c) first_w_.b[c] = bi->second[c];
+    }
     layers_[sp.name] = L;
   }
   if (num_output_channels > cnet_) { err = "the network produces fewer channels than num_output_channels"; return false; }
@@ -207,18 +203,15 @@ int Network::forward_cp8(const void* chunk, int in_dtype, Int3 cs, const PatchPo
   {
     const ConvLayer& L = layers_.at("enc0.0");
     prof_begin("enc0.0", s);
-    if (chunk && in_dtype == CFB_DTYPE_U8 && L.packed.w_ts && !getenv("CFB_SIMT_FIRST_CONV") && !getenv("CFB_UMMA_FIRST_CONV"))
-      launch_first_conv_ts(chunk, cs, patches, nb, s0, L.packed, h_e0a_, P, s);
-    else if (chunk && in_dtype == CFB_DTYPE_U8 && getenv("CFB_UMMA_FIRST_CONV") && P != kFmtF16F8) launch_first_conv_umma(chunk, cs, patches, nb, s0, L.packed, h_e0a_, s);
-    else if (chunk) launch_first_conv_cp8(chunk, in_dtype, cs, patches, nb, s0, L.w, L.bias, h_e0a_, P, s,
-                                          getenv("CFB_FIRST_CONV_SMEM_W") ? nullptr : &first_w_);
+    if (chunk) launch_first_conv_cp8(chunk, in_dtype, cs, patches, nb, s0, L.w, L.bias, h_e0a_, P, s,
+                                     getenv("CFB_FIRST_CONV_SMEM_W") ? nullptr : &first_w_);
     else launch_first_conv_cp8_from_patches(buf_in_, nb, s0, L.w, L.bias, h_e0a_, P, s);
     prof_end(s);
   }
   auto conv = [&](const char* name, const __half* a, int ca, const __half* b, int cb, __half* out, Int3 sz, __half* pool_out = nullptr) {
     const ConvLayer& L = layers_.at(name);
     prof_begin(name, s);
-    launch_conv3_umma(a, ca, b, cb, L.packed, out, nb, sz, /*relu=*/true, s, nullptr, pool_out);
+    launch_conv3_wgmma(a, ca, b, cb, L.packed, out, nb, sz, /*relu=*/true, s, nullptr, pool_out);
     prof_end(s);
   };
   // the two encoder outputs feed a (1,2,2) max pool: fused into the convolution's epilogue unless CFB_NO_POOL_FUSION is set
@@ -231,20 +224,21 @@ int Network::forward_cp8(const void* chunk, int in_dtype, Int3 cs, const PatchPo
   if (!fuse_pool) { prof_begin("pool1", s); launch_maxpool_cp8(h_e1_, h_p1_, 32, P, nb, s1, s); prof_end(s); } else ++launches_saved;
   conv("enc2.0", h_p1_, 32, nullptr, 0, h_e2a_, s2);
   conv("enc2.2", h_e2a_, 64, nullptr, 0, h_e2_, s2);
+  // transposed convolutions on wgmma; CFB_SIMT_CONVT selects the CUDA-core kernel (fp32 math, a cross-check)
   const bool simt_up = getenv("CFB_SIMT_CONVT") != nullptr;
   { const ConvLayer& L = layers_.at("up1"); prof_begin("up1", s);
-    if (simt_up) launch_convT_cp8(h_e2_, L.w, L.bias, h_u1_, 64, 32, P, nb, s2, s); else launch_convT_umma(h_e2_, L.packed, h_u1_, nb, s2, s);
+    if (simt_up) launch_convT_cp8(h_e2_, L.w, L.bias, h_u1_, 64, 32, P, nb, s2, s); else launch_convT_wgmma(h_e2_, L.packed, h_u1_, nb, s2, s);
     prof_end(s); }
   conv("dec1.0", h_u1_, 32, h_e1_, 32, h_d1a_, s1);  // torch.cat([up1, enc1])
   conv("dec1.2", h_d1a_, 32, nullptr, 0, h_d1_, s1);
   { const ConvLayer& L = layers_.at("up0"); prof_begin("up0", s);
-    if (simt_up) launch_convT_cp8(h_d1_, L.w, L.bias, h_u0_, 32, 16, P, nb, s1, s); else launch_convT_umma(h_d1_, L.packed, h_u0_, nb, s1, s);
+    if (simt_up) launch_convT_cp8(h_d1_, L.w, L.bias, h_u0_, 32, 16, P, nb, s1, s); else launch_convT_wgmma(h_d1_, L.packed, h_u0_, nb, s1, s);
     prof_end(s); }
   conv("dec0.0", h_u0_, 16, h_e0_, 16, h_d0a_, s0);  // torch.cat([up0, enc0])
   if (tail) {  // 3x3x3 conv + ReLU + 1x1x1 head + sigmoid + crop + bump mask + blend in one kernel
     const ConvLayer& L = layers_.at("dec0.2");
     prof_begin("dec0.2+head+blend", s);
-    launch_conv3_umma(h_d0a_, 16, nullptr, 0, L.packed, h_d0_, nb, s0, /*relu=*/true, s, tail);
+    launch_conv3_wgmma(h_d0a_, 16, nullptr, 0, L.packed, h_d0_, nb, s0, /*relu=*/true, s, tail);
     prof_end(s);
     return 14 - launches_saved;
   }
@@ -317,7 +311,7 @@ int Network::debug_conv3(const float* h_in, int cin, Int3 size, const float* h_w
   CFB_CUDA(cudaMemcpyAsync(d_w, h_w, (size_t)cout * cin * 27 * 4, cudaMemcpyHostToDevice, s));
   CFB_CUDA(cudaMemcpyAsync(d_b, h_b, (size_t)cout * 4, cudaMemcpyHostToDevice, s));
   if (umma()) {
-    if (cin % 16) { cudaFree(d_in); cudaFree(d_w); cudaFree(d_b); cudaFree(d_out); throw std::runtime_error("tcgen05 conv needs cin % 16 == 0"); }
+    if (cin % 16) { cudaFree(d_in); cudaFree(d_w); cudaFree(d_b); cudaFree(d_out); throw std::runtime_error("the wgmma convolution needs cin % 16 == 0"); }
     const int P = parts();
     __half *c_in = nullptr, *c_out = nullptr;
     CFB_CUDA(cudaMalloc(&c_in, (size_t)cin * P * v * 2));
@@ -327,7 +321,7 @@ int Network::debug_conv3(const float* h_in, int cin, Int3 size, const float* h_w
     launch_planar_to_cp8(d_in, c_in, cin, fmt(), 1, size, s);
     // exercise the two-source (concat) path whenever the channel count allows it
     const int ca = cin >= 32 ? cin / 2 : cin, cb = cin - ca;
-    launch_conv3_umma(c_in, ca, cb ? c_in + (size_t)ca * P * v : nullptr, cb, pk, c_out, 1, size, relu, s);
+    launch_conv3_wgmma(c_in, ca, cb ? c_in + (size_t)ca * P * v : nullptr, cb, pk, c_out, 1, size, relu, s);
     launch_cp8_to_planar(c_out, d_out, cout, fmt(), 1, size, s);
     CFB_CUDA(cudaMemcpyAsync(h_out, d_out, (size_t)cout * v * 4, cudaMemcpyDeviceToHost, s));
     cudaError_t err = cudaStreamSynchronize(s);

@@ -7,7 +7,7 @@
 #include <vector>
 
 #include "common.cuh"
-#include "kernels_umma.cuh"
+#include "kernels_conv.cuh"
 
 namespace cfb {
 
@@ -16,7 +16,7 @@ struct ConvLayer {
   int cin = 0, cout = 0;
   float* w = nullptr;     // fp32, state_dict layout
   float* bias = nullptr;  // fp32
-  PackedConv packed;      // fp16 (hi/lo) B-operand blocks for the tcgen05 path (3x3x3 layers, cin >= 16)
+  PackedConv packed;      // B-operand blocks for the wgmma path (3x3x3 layers, cin >= 16)
 };
 
 class Network {
@@ -31,7 +31,7 @@ class Network {
   int forward_from_chunk(const void* chunk, int in_dtype, Int3 chunk_size, const PatchPos* patches, int nb,
                          cudaStream_t s);
   int forward_from_host_patches(const float* h_patches, int nb, cudaStream_t s);
-  // Whole-chunk path: extract + network + crop + bump mask + accumulate into the output chunk.  On the tcgen05
+  // Whole-chunk path: extract + network + crop + bump mask + accumulate into the output chunk.  On the wgmma
   // path the head and the blend are fused into the epilogue of the last convolution.
   int forward_and_blend(const void* chunk, int in_dtype, Int3 chunk_size, const PatchPos* patches, int nb, Int3 out_patch,
                         Int3 crop, const float* mask, float* out, int channels, Int3 out_size, float scale, cudaStream_t s);
@@ -51,11 +51,11 @@ class Network {
  private:
   void allocate();
   int forward(int nb, cudaStream_t s);  // from buf_in_ (fp32 SIMT path)
-  // tcgen05 path: chunk != nullptr -> first layer reads the chunk, else the staged fp32 patches in buf_in_
+  // wgmma path: chunk != nullptr -> first layer reads the chunk, else the staged fp32 patches in buf_in_
   int forward_cp8(const void* chunk, int in_dtype, Int3 chunk_size, const PatchPos* patches, int nb, cudaStream_t s,
                   bool with_head, const ConvTail* tail = nullptr);
   bool umma() const { return precision_ != 0; }
-  // activation number format of the tcgen05 path (act_format.cuh) and its planes per 8-channel chunk
+  // activation number format of the wgmma path (act_format.cuh) and its planes per 8-channel chunk
   int fmt() const { return precision_ == 1 ? kFmtF16x2 : (precision_ == 3 ? kFmtF16F8 : kFmtF16); }
   int parts() const { return fmt_planes(fmt()); }
 
@@ -82,7 +82,7 @@ class Network {
   float *buf_in_ = nullptr, *e0a_ = nullptr, *e0_ = nullptr, *p0_ = nullptr, *e1a_ = nullptr, *e1_ = nullptr,
         *p1_ = nullptr, *e2a_ = nullptr, *e2_ = nullptr, *u1_ = nullptr, *d1a_ = nullptr, *d1_ = nullptr,
         *u0_ = nullptr, *d0a_ = nullptr, *d0_ = nullptr, *net_out_ = nullptr;
-  // CP8 fp16 activations of the tcgen05 path
+  // CP8 fp16 activations of the wgmma path
   __half *h_e0a_ = nullptr, *h_e0_ = nullptr, *h_p0_ = nullptr, *h_e1a_ = nullptr, *h_e1_ = nullptr, *h_p1_ = nullptr,
          *h_e2a_ = nullptr, *h_e2_ = nullptr, *h_u1_ = nullptr, *h_d1a_ = nullptr, *h_d1_ = nullptr, *h_u0_ = nullptr,
          *h_d0a_ = nullptr, *h_d0_ = nullptr;

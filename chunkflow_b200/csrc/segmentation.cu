@@ -182,7 +182,7 @@ int guarded_seg(F&& f) {
 
 int grid_for(int64_t items) {
   int64_t b = ceil_div64(items, kT);
-  return (int)std::max<int64_t>(1, std::min<int64_t>(b, 148 * 16));
+  return (int)std::max<int64_t>(1, std::min<int64_t>(b, 132 * 16));
 }
 
 }  // namespace

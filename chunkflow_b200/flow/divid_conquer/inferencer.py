@@ -1,4 +1,4 @@
-"""Chunk-level overlap-tile convnet inference on a B200.
+"""Chunk-level overlap-tile convnet inference on an H100.
 
 Drop-in for the reference's ``Inferencer``
 (chunkflow/flow/divid_conquer/inferencer.py:21-479): same constructor keywords, same
@@ -7,7 +7,7 @@ chunk is uploaded once, every patch is extracted, run through the network, bump-
 and blended by CUDA kernels on the device, and the normalised result is downloaded once.
 
 Frameworks:
-  'b200'      the fixed 3-level U-Net (chunkflow_b200/convnet/unet3l.py) as sm_100a kernels.
+  'b200'      the fixed 3-level U-Net (chunkflow_b200/convnet/unet3l.py) as sm_90a kernels.
   'pytorch'   accepted when the model file is that canonical U-Net (the same file drives the
               reference's ``-f pytorch`` CPU path, the parity oracle); any other torch model
               is refused -- there is no CPU / eager fallback.
@@ -158,7 +158,7 @@ class Inferencer(object):
     def _patches_in_flight(self, framework_code) -> int:
         """``batch_size`` is a scheduling hint here (the reference asserts 1 for pytorch although its examples pass
         12, inferencer.py:216-220).  With the default of 1 the device network path picks the number of patches in
-        flight itself: enough CTAs to fill 148 SMs at every U-Net level, bounded by a quarter of the free memory
+        flight itself: enough CTAs to fill 132 SMs at every U-Net level, bounded by a quarter of the free memory
         (about 540 bytes of fp16 hi/lo activations per patch voxel)."""
         if self.batch_size > 1 or framework_code != _native.FRAMEWORK_UNET3L:
             return self.batch_size

@@ -1,4 +1,4 @@
-"""Patch backends that run on the B200 through the C-ABI.
+"""Patch backends that run on the GPU through the C-ABI.
 
 ``B200``     : the fixed 3-level U-Net forward + crop + bump mask on the device, with the
                per-patch numpy API of the reference's ``PyTorch`` backend
@@ -56,11 +56,11 @@ def load_state_dict(convnet_model=None, convnet_weight_path=None) -> dict:
 def precision_code(dtype: str = "float32", precision=None) -> int:
     """``--dtype`` -> precision mode of the convolution stack.
 
-    float32 -> 'f16f8' (default): tcgen05 tensor cores, fp16 main product plus ONE e4m3 product of twice the K depth that
+    float32 -> 'f16f8' (default): wgmma tensor cores, fp16 main product plus ONE e4m3 product of twice the K depth that
     carries both hi/lo correction terms, fp32 accumulation -- two tensor-core products per multiply (csrc/act_format.cuh);
-    measured 1.7e-4 .. 2.1e-4 max-abs against the fp32 CPU reference (the bar is 1e-3).
-    'f16x3': fp16 hi/lo split operands, three products per multiply, 3e-5 .. 5e-5 max-abs, ~9 % slower.
-    float16 -> 'f16': single-pass fp16 tensor cores, ~3e-3 max-abs (the reference documents float16 as a lower-precision
+    the tests assert <= 5e-4 max-abs against the fp32 CPU reference (the bar is 1e-3).
+    'f16x3': fp16 hi/lo split operands, three products per multiply, asserted <= 2e-4.
+    float16 -> 'f16': single-pass fp16 tensor cores, asserted <= 2e-2 (the reference documents float16 as a lower-precision
     option, flow.py:1871-1874).  ``precision`` (or env CHUNKFLOW_B200_PRECISION) forces one of 'simt' (fp32 FFMA on CUDA
     cores), 'f16x3', 'f16f8', 'f16'.
     """

@@ -1,5 +1,5 @@
 /*
- * chunkflow_b200 -- C-ABI of the B200-native `inference` hot path.
+ * chunkflow_b200 -- C-ABI of the H100-native `inference` hot path.
  *
  * Drop-in boundary for chunkflow's overlap-tile convnet inference.  The reference is
  * pure Python; each entry point names the reference interface it replaces
@@ -52,9 +52,9 @@ extern "C" {
 
 /* precision of the convolution stack */
 #define CFB_PRECISION_F32_SIMT 0   /* fp32 FFMA direct convolution (exact-order-free fp32) */
-#define CFB_PRECISION_F16X3_UMMA 1 /* tcgen05 fp16 hi/lo split, fp32 accumulate (~fp32 accuracy) */
-#define CFB_PRECISION_F16_UMMA 2   /* tcgen05 single-pass fp16, fp32 accumulate (reference --dtype float16) */
-#define CFB_PRECISION_F16F8_UMMA 3 /* tcgen05 fp16 main product + ONE e4m3 (K = 32) product carrying both correction terms,
+#define CFB_PRECISION_F16X3_UMMA 1 /* wgmma fp16 hi/lo split, fp32 accumulate (~fp32 accuracy) */
+#define CFB_PRECISION_F16_UMMA 2   /* wgmma single-pass fp16, fp32 accumulate (reference --dtype float16) */
+#define CFB_PRECISION_F16F8_UMMA 3 /* wgmma fp16 main product + ONE e4m3 (K = 32) product carrying both correction terms,
                                       fp32 accumulate: two tensor-core products per multiply instead of f16x3's three
                                       (csrc/act_format.cuh) */
 

@@ -13,7 +13,7 @@ MODEL_FILE = os.path.join(ROOT, "chunkflow_b200", "convnet", "unet3l.py")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "slow: minutes of CPU oracle time (still part of `-m gpu`)")
 
 

@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 BLEND_ATOL = 2e-6
 # fp32 SIMT convolutions vs torch-CPU: different summation order only
 NET_ATOL_SIMT = 2e-5
-# default mode 'f16f8' (tcgen05: fp16 main product + one e4m3 K=32 product carrying both hi/lo correction terms, fp32
+# default mode 'f16f8' (wgmma: fp16 main product + one e4m3 K=32 product carrying both hi/lo correction terms, fp32
 # accumulate): measured 0.9e-4 .. 2.1e-4; the bar in BASELINE.json's north_star is 1e-3 max-abs -- assert 2x tighter
 NET_ATOL_F32 = 5e-4
 # 'f16x3' (fp16 hi/lo split, three products per multiply): measured 2e-5 .. 5e-5 -- assert 5x tighter than the bar
@@ -49,7 +49,7 @@ def test_identity_nonaligned_golden(golden):
     np.testing.assert_allclose(out.array, g["output"], rtol=0, atol=BLEND_ATOL)
     got = [[[s.start, s.stop] for s in pair[0]] + [[s.start, s.stop] for s in pair[1]] for pair in inf.patch_slices_list]
     assert got == g["patch_slices"].tolist()
-    assert "B200" in inf.compute_device or "NVIDIA" in inf.compute_device
+    assert "H100" in inf.compute_device or "NVIDIA" in inf.compute_device
 
 
 def test_identity_aligned_golden(golden):
@@ -156,7 +156,7 @@ UMMA_CASES = [(16, 16, (3, 8, 40)), (16, 16, (4, 16, 70)), (32, 32, (3, 12, 20))
 
 @pytest.mark.parametrize("cin,cout,size", UMMA_CASES)
 def test_conv3_layer_tcgen05_split_against_torch(cin, cout, size):
-    # hi/lo split operands: ~22 significant bits, fp32 accumulation in TMEM
+    # hi/lo split operands: ~22 significant bits, fp32 accumulation
     _conv3_case(_native.PRECISION_F16X3_UMMA, cin, cout, size, 5e-5)
 
 
@@ -164,8 +164,8 @@ def test_conv3_layer_tcgen05_split_against_torch(cin, cout, size):
 @pytest.mark.parametrize("cin,cout,size", [(16, 16, (3, 8, 40)), (16, 16, (9, 16, 70)), (32, 32, (5, 12, 20)), (16, 32, (4, 6, 128)),
                                            (32, 16, (7, 8, 130)), (64, 32, (4, 16, 16)), (16, 16, (1, 7, 9))])
 def test_conv3_layer_tcgen05_zstacked_kernel(monkeypatch, zstack, cin, cout, size):
-    """The z-stacked kernel variant (T output planes per job, dz taps stacked along N), forced."""
-    monkeypatch.setenv("CFB_FORCE_ZSTACK", zstack)
+    """The convolution split along z into blocks of T output planes per CTA (each block loads its own halo planes), forced."""
+    monkeypatch.setenv("CFB_FORCE_ZBLOCK", zstack)
     _conv3_case(_native.PRECISION_F16X3_UMMA, cin, cout, size, 5e-5)
     if cin == 16:
         _conv3_case(_native.PRECISION_F16_UMMA, cin, cout, size, 1e-2)
@@ -175,9 +175,10 @@ def test_conv3_layer_tcgen05_zstacked_kernel(monkeypatch, zstack, cin, cout, siz
 @pytest.mark.parametrize("cin,cout,size", [(16, 16, (3, 8, 40)), (16, 16, (9, 16, 70)), (32, 32, (5, 12, 20)), (16, 32, (4, 6, 128)),
                                            (32, 16, (7, 8, 130)), (64, 32, (4, 16, 16)), (16, 16, (1, 7, 9))])
 def test_conv3_layer_tcgen05_tmem_shift_kernel(monkeypatch, zstack, cin, cout, size):
-    """z-stacked + TMEM-resident activation tile: MMA(dx=0), tcgen05.shift, MMA(dx=1), shift, MMA(dx=2)."""
-    monkeypatch.setenv("CFB_FORCE_ZSTACK", zstack)
-    monkeypatch.setenv("CFB_FORCE_TSHIFT", "1")
+    """z blocks of T output planes with the weights streamed through a 3-stage ring (taps refilled while the MMAs run)
+    instead of resident, forced."""
+    monkeypatch.setenv("CFB_FORCE_ZBLOCK", zstack)
+    monkeypatch.setenv("CFB_FORCE_WEIGHT_RING", "1")
     _conv3_case(_native.PRECISION_F16X3_UMMA, cin, cout, size, 5e-5)
     if cin == 16:
         _conv3_case(_native.PRECISION_F16_UMMA, cin, cout, size, 1e-2)
@@ -193,7 +194,7 @@ def test_conv3_layer_tcgen05_f16f8_against_torch(cin, cout, size):
 @pytest.mark.parametrize("zstack", ["2", "3", "4"])
 @pytest.mark.parametrize("cin,cout,size", [(16, 16, (9, 16, 70)), (32, 32, (5, 12, 20)), (64, 32, (4, 16, 16)), (16, 16, (1, 7, 9))])
 def test_conv3_layer_f16f8_forced_zstack(monkeypatch, zstack, cin, cout, size):
-    monkeypatch.setenv("CFB_FORCE_ZSTACK", zstack)
+    monkeypatch.setenv("CFB_FORCE_ZBLOCK", zstack)
     _conv3_case(_native.PRECISION_F16F8_UMMA, cin, cout, size, 4e-4)
 
 
@@ -325,7 +326,7 @@ def test_cli_readme_example(golden):
     task = res.return_value[0]
     out = task["chunk"]
     assert out.shape == (3, 40, 256, 256) and 0 < out.array.min() and out.array.max() < 1
-    assert "inference" in task["log"]["timer"] and "B200" in task["log"]["compute_device"]
+    assert "inference" in task["log"]["timer"] and "H100" in task["log"]["compute_device"]
 
 
 def test_slab_entry_point_matches_whole_chunk():
@@ -497,21 +498,22 @@ def test_host_plugin_shape_errors_and_myelin_zero_threshold():
 
 
 def test_kernel_variants_agree(monkeypatch, unet_model):
-    """Every tcgen05 kernel variant computes the same network: fused vs unfused tail, CUDA-core vs (experimental, latency-bound) tensor-core
-    first layer, tensor-core vs CUDA-core transposed convolutions, z-stacked vs per-tap 3x3x3 kernel (forced through env switches)."""
+    """Every kernel variant computes the same network: fused vs unfused head+blend tail, first layer with its weights in the constant
+    bank vs in shared memory, 3x3x3 convolutions split into z blocks, weights streamed through a ring, pooling fused into the
+    convolution epilogue vs its own kernel, tensor-core vs CUDA-core transposed convolutions (forced through env switches)."""
     rng = np.random.default_rng(31)
     img = rng.integers(0, 256, size=(20, 96, 104), dtype=np.uint8)
     kw = dict(input_patch_size=(16, 64, 64), output_patch_overlap=(4, 16, 16), num_output_channels=3, framework="b200",
-              batch_size=5, precision="f16x3")   # (the f16f8 mode exists on the TMEM-shift kernel only)
+              batch_size=5, precision="f16x3")
     ref, _ = O.infer_chunk(img, input_patch_size=(16, 64, 64), output_patch_overlap=(4, 16, 16), num_output_channels=3,
                            framework="pytorch", model=unet_model)
     results = {}
-    for name, env in [("default", {}), ("unfused_tail", {"CFB_NO_FUSED_TAIL": "1"}), ("umma_first", {"CFB_UMMA_FIRST_CONV": "1"}),
-                      ("simt_first", {"CFB_SIMT_FIRST_CONV": "1"}),
-                      ("simt_convT", {"CFB_SIMT_CONVT": "1"}), ("per_tap", {"CFB_NO_ZSTACK": "1"}), ("zstack4", {"CFB_FORCE_ZSTACK": "4"}),
-                      ("no_shift", {"CFB_NO_TSHIFT": "1"}), ("shift2", {"CFB_FORCE_ZSTACK": "2", "CFB_FORCE_TSHIFT": "1"})]:
-        for k in ("CFB_NO_FUSED_TAIL", "CFB_UMMA_FIRST_CONV", "CFB_SIMT_FIRST_CONV", "CFB_SIMT_CONVT", "CFB_NO_ZSTACK", "CFB_FORCE_ZSTACK",
-                  "CFB_NO_TSHIFT", "CFB_FORCE_TSHIFT"):
+    for name, env in [("default", {}), ("unfused_tail", {"CFB_NO_FUSED_TAIL": "1"}), ("smem_first", {"CFB_FIRST_CONV_SMEM_W": "1"}),
+                      ("zblock4", {"CFB_FORCE_ZBLOCK": "4"}), ("weight_ring", {"CFB_FORCE_WEIGHT_RING": "1"}),
+                      ("zblock2_ring", {"CFB_FORCE_ZBLOCK": "2", "CFB_FORCE_WEIGHT_RING": "1"}),
+                      ("unfused_pool", {"CFB_NO_POOL_FUSION": "1"}), ("simt_convT", {"CFB_SIMT_CONVT": "1"})]:
+        for k in ("CFB_NO_FUSED_TAIL", "CFB_FIRST_CONV_SMEM_W", "CFB_FORCE_ZBLOCK", "CFB_FORCE_WEIGHT_RING", "CFB_NO_POOL_FUSION",
+                  "CFB_SIMT_CONVT"):
             monkeypatch.delenv(k, raising=False)
         for k, v in env.items():
             monkeypatch.setenv(k, v)
@@ -524,15 +526,18 @@ def test_kernel_variants_agree(monkeypatch, unet_model):
 
 
 def test_f16f8_unfused_and_cuda_core_paths(monkeypatch, unet_model):
-    """The default f16f8 number format through the kernels that are not on the default route: the unfused head+blend tail and the
-    CUDA-core transposed convolution (they decode / encode the H + A8 + L8 records through load8 / store8, kernels_cp8.cu)."""
+    """The default f16f8 number format through the kernels that are not on the default route: the unfused head+blend tail, the
+    first layer with shared-memory weights, the stand-alone pool and the CUDA-core transposed convolution (they decode / encode the
+    H + A8 + L8 records through load8 / store8, kernels_cp8.cu)."""
     rng = np.random.default_rng(41)
     img = rng.integers(0, 256, size=(20, 96, 104), dtype=np.uint8)
     kw = dict(input_patch_size=(16, 64, 64), output_patch_overlap=(4, 16, 16), num_output_channels=3, framework="b200", batch_size=5)
     ref, _ = O.infer_chunk(img, input_patch_size=(16, 64, 64), output_patch_overlap=(4, 16, 16), num_output_channels=3,
                            framework="pytorch", model=unet_model)
-    for env in ({}, {"CFB_NO_FUSED_TAIL": "1"}, {"CFB_SIMT_CONVT": "1"}, {"CFB_FORCE_ZSTACK": "2"}, {"CFB_SIMT_FIRST_CONV": "1"}):
-        for k in ("CFB_NO_FUSED_TAIL", "CFB_SIMT_CONVT", "CFB_FORCE_ZSTACK", "CFB_SIMT_FIRST_CONV"):
+    for env in ({}, {"CFB_NO_FUSED_TAIL": "1"}, {"CFB_FIRST_CONV_SMEM_W": "1"}, {"CFB_FORCE_ZBLOCK": "2"}, {"CFB_FORCE_WEIGHT_RING": "1"},
+                {"CFB_NO_POOL_FUSION": "1"}, {"CFB_SIMT_CONVT": "1"}):
+        for k in ("CFB_NO_FUSED_TAIL", "CFB_FIRST_CONV_SMEM_W", "CFB_FORCE_ZBLOCK", "CFB_FORCE_WEIGHT_RING", "CFB_NO_POOL_FUSION",
+                  "CFB_SIMT_CONVT"):
             monkeypatch.delenv(k, raising=False)
         for k, v in env.items():
             monkeypatch.setenv(k, v)

@@ -39,7 +39,7 @@ def main():
     ap.add_argument("--threshold", type=float, default=0.5)
     args = ap.parse_args()
     n, z = args.size, args.z
-    peak = 6584.5
+    peak = 3350.0   # H100 SXM data sheet HBM3 GB/s
     try:
         peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
     except Exception:

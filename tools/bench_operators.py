@@ -1,4 +1,4 @@
-"""Achieved HBM bandwidth of the operators either side of `inference` (SURVEY section 8 f3) on one B200:
+"""Achieved HBM bandwidth of the operators either side of `inference` (SURVEY section 8 f3) on one GPU:
 algorithmic bytes / CUDA-event time, against MEASURED_PEAKS.json `hbm_gbs`.  One JSON line.
 
     python tools/bench_operators.py [--size 1024]
@@ -32,7 +32,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--size", type=int, default=1024)
     n = ap.parse_args().size
-    peak = 6650.0
+    peak = 3350.0   # H100 SXM data sheet HBM3 GB/s
     try:
         peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
     except Exception:

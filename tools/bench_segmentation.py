@@ -22,7 +22,7 @@ def main():
     ap.add_argument("--size", type=int, default=512)
     args = ap.parse_args()
     n = args.size
-    peak = 6584.5
+    peak = 3350.0   # H100 SXM data sheet HBM3 GB/s
     try:
         peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
     except Exception:
