@@ -16,7 +16,7 @@ OK = 0
 ERR_INVALID_ARGUMENT, ERR_CUDA, ERR_WEIGHTS, ERR_OUTPUT_RANGE, ERR_UNSUPPORTED, ERR_CAPACITY = -1, -2, -3, -4, -5, -6
 FRAMEWORK_UNET3L, FRAMEWORK_IDENTITY = 0, 1
 PRECISION_F32_SIMT, PRECISION_F16X3_UMMA, PRECISION_F16_UMMA, PRECISION_F16F8_UMMA = 0, 1, 2, 3
-DTYPE_U8, DTYPE_F32, DTYPE_U32 = 0, 1, 2
+DTYPE_U8, DTYPE_F32, DTYPE_U32, DTYPE_U64 = 0, 1, 2, 3
 AUGMENT_NONE, AUGMENT_REFERENCE, AUGMENT_SPATIAL = 0, 1, 2
 QUANTIZE_XY, QUANTIZE_Z = 0, 1
 
@@ -32,6 +32,7 @@ EXPORTS = (
     "cfb_connected_components_device", "cfb_connected_components_workspace",
     "cfb_watershed_workspace", "cfb_watershed_device", "cfb_region_graph_workspace", "cfb_region_graph_device",
     "cfb_region_graph_read", "cfb_agglomerate_edges_host", "cfb_relabel_device",
+    "cfb_evaluate_workspace", "cfb_contingency_device", "cfb_contingency_scores", "cfb_contingency_read",
 )
 
 
@@ -44,6 +45,22 @@ class Params(C.Structure):
         ("mask_output_chunk", C.c_int32), ("augment", C.c_int32), ("has_myelin_threshold", C.c_int32),
         ("mask_myelin_threshold", C.c_float), ("check_output_range", C.c_int32),
     ]
+
+
+class SegScores(C.Structure):
+    """cfb_seg_scores: the statistics of a contingency table and the five scores of one size threshold."""
+    _fields_ = [
+        ("struct_size", C.c_int32), ("reserved", C.c_int32),
+        ("n", C.c_uint64), ("sum_sq_pairs", C.c_uint64), ("sum_sq_rows", C.c_uint64), ("sum_sq_cols", C.c_uint64),
+        ("n_both_nonzero", C.c_uint64), ("seg_ids", C.c_uint64), ("gt_ids", C.c_uint64), ("pairs", C.c_uint64),
+        ("pairs_over_threshold", C.c_uint64),
+        ("size_threshold", C.c_double), ("xlog_pairs", C.c_double), ("xlog_rows", C.c_double), ("xlog_cols", C.c_double),
+        ("rand_index", C.c_double), ("adjusted_rand_index", C.c_double), ("variation_of_information", C.c_double),
+        ("fowlkes_mallows_index", C.c_double), ("false_merges", C.c_double), ("false_splits", C.c_double),
+    ]
+
+    def as_dict(self) -> dict:
+        return {name: getattr(self, name) for name, _ in self._fields_ if name not in ("struct_size", "reserved")}
 
 
 class NativeError(RuntimeError):
@@ -126,6 +143,11 @@ def load() -> C.CDLL:
     lib.cfb_region_graph_read.argtypes = [vp, i64, i64, vp, vp, vp, vp, vp]
     lib.cfb_agglomerate_edges_host.argtypes = [i64, i64, vp, vp, vp, vp, C.c_float, vp]
     lib.cfb_relabel_device.argtypes = [vp, i64, vp, i64, vp, vp]
+    lib.cfb_evaluate_workspace.argtypes = [i64]
+    lib.cfb_evaluate_workspace.restype = i64
+    lib.cfb_contingency_device.argtypes = [vp, i32, vp, i32, i64, i64, i64, vp, i64, C.POINTER(i64), vp]
+    lib.cfb_contingency_scores.argtypes = [vp, i64, C.c_double, C.POINTER(SegScores), vp]
+    lib.cfb_contingency_read.argtypes = [vp, i64, i64, vp, vp, vp, vp]
     for name in EXPORTS:
         getattr(lib, name)   # every declared symbol must be there
     _lib = lib
@@ -230,6 +252,36 @@ def agglomerate_edges_host(num_nodes: int, u, v, sum_fixed, count, threshold: fl
 def relabel_device(d_labels: int, n: int, d_map: int, map_size: int, d_out: int, stream: int = 0) -> None:
     check(load().cfb_relabel_device(C.c_void_p(d_labels), int(n), C.c_void_p(d_map), int(map_size), C.c_void_p(d_out),
                                     C.c_void_p(stream)))
+
+
+# ---- `evaluate-segmentation` (include/chunkflow_b200.h, DESIGN.md section 0, row f5) ----
+def evaluate_workspace(table_slots: int) -> int:
+    return int(load().cfb_evaluate_workspace(int(table_slots)))
+
+
+def contingency_device(d_seg: int, seg_dtype: int, d_gt: int, gt_dtype: int, zyx, d_workspace: int, table_slots: int,
+                       stream: int = 0) -> int:
+    """-> number of (seg id, gt id) pairs; raises NativeError with code ERR_CAPACITY when the table is too small."""
+    n = C.c_int64()
+    check(load().cfb_contingency_device(C.c_void_p(d_seg), int(seg_dtype), C.c_void_p(d_gt), int(gt_dtype), *(int(v) for v in zyx),
+                                        C.c_void_p(d_workspace), int(table_slots), C.byref(n), C.c_void_p(stream)))
+    return int(n.value)
+
+
+def contingency_scores(d_workspace: int, table_slots: int, size_threshold: float, stream: int = 0) -> SegScores:
+    out = SegScores()
+    out.struct_size = C.sizeof(SegScores)
+    check(load().cfb_contingency_scores(C.c_void_p(d_workspace), int(table_slots), float(size_threshold), C.byref(out),
+                                        C.c_void_p(stream)))
+    return out
+
+
+def contingency_read(d_workspace: int, table_slots: int, num_pairs: int, stream: int = 0):
+    """-> (seg ids uint64, gt ids uint64, counts uint32) host arrays sorted by (seg, gt)."""
+    s, g, c = np.empty(num_pairs, np.uint64), np.empty(num_pairs, np.uint64), np.empty(num_pairs, np.uint32)
+    check(load().cfb_contingency_read(C.c_void_p(d_workspace), int(table_slots), int(num_pairs), _ptr(s), _ptr(g), _ptr(c),
+                                      C.c_void_p(stream)))
+    return s, g, c
 
 
 def device_memory(device: int = 0) -> tuple:

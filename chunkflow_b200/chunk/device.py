@@ -11,6 +11,7 @@ bookkeeping of the reference's ``Chunk`` and mirrors, name for name, the referen
     quantize             reference chunk/affinity_map/base.py:33-57     (AffinityMap)
     connected_component  reference chunk/base.py:128-137                (Chunk -> cc3d)
     agglomerate          reference plugins/agglomerate.py:8-48          (plugin -> waterz)
+    evaluate             reference chunk/segmentation.py:33-67          (Segmentation -> gala, lib/gala/evaluate.py)
 
 so that ``create-chunk | normalize-contrast | inference | crop-margin | quantize`` moves the image to the GPU once and
 brings a uint8 thumbnail (or nothing) back instead of the 12-byte-per-voxel affinity map.  There is no CPU fallback.
@@ -304,6 +305,78 @@ class DeviceChunk:
         out.num_fragments, out.num_edges = num, int(u.size)
         out.num_components = int(np.count_nonzero(root[1:] == np.arange(1, root.size, dtype=np.uint32)))
         return out
+
+    # ---- Segmentation.evaluate: contingency table + gala's scores -----------------------------------
+    def _label_tensor(self):
+        """(tensor, dtype code) of a (z,y,x) label volume.  Repository convention: int32 holds uint32 values and int64 the
+        uint64 bit pattern (what numpy's astype(np.uint64) gives a signed array) -- every score is invariant under this
+        one-to-one relabelling."""
+        torch = _torch()
+        t = self.tensor
+        if t.ndim == 4:
+            assert t.shape[0] == 1, "a segmentation has one channel"
+            t = t[0]
+        codes = {torch.uint8: _native.DTYPE_U8, torch.bool: _native.DTYPE_U8, torch.int32: _native.DTYPE_U32,
+                 torch.int64: _native.DTYPE_U64}
+        for name, code in (("uint32", _native.DTYPE_U32), ("uint64", _native.DTYPE_U64)):
+            if hasattr(torch, name):
+                codes[getattr(torch, name)] = code
+        if t.dtype not in codes:
+            raise TypeError(f"a label volume on the device is uint8, int32 / uint32 or int64 / uint64, not {t.dtype}")
+        if t.numel() >= 2 ** 32 - 1:
+            raise ValueError("more than 2^32 - 1 voxels")
+        return t.contiguous(), codes[t.dtype]
+
+    def _contingency(self, groundtruth: "DeviceChunk", table_slots: Optional[int] = None):
+        """(workspace, slots, pairs): the contingency table of self (rows) and ``groundtruth`` (columns) built on the device.
+        The table starts at ``table_slots`` (default: from the voxel count) and is grown on overflow."""
+        torch = _torch()
+        s, sc = self._label_tensor()
+        g, gc = groundtruth._label_tensor()
+        if tuple(s.shape) != tuple(g.shape) or s.device != g.device:
+            raise ValueError(f"segmentation {tuple(s.shape)} and ground truth {tuple(g.shape)} must have the same shape and device")
+        slots = int(table_slots) if table_slots is not None else 1 << max(10, min(24, (s.numel() // 64).bit_length()))
+        with self._on_device():
+            while True:
+                work = torch.empty(_native.evaluate_workspace(slots), dtype=torch.uint8, device=s.device)
+                try:
+                    n = _native.contingency_device(s.data_ptr(), sc, g.data_ptr(), gc, tuple(s.shape), work.data_ptr(), slots,
+                                                   self._stream())
+                    if 2 * n <= slots:
+                        return work, slots, n
+                except _native.NativeError as err:
+                    if err.code != _native.ERR_CAPACITY:
+                        raise
+                del work
+                slots <<= 2          # too full (or more than half full: long probe sequences): a larger table
+                if slots >= 1 << 31:
+                    raise RuntimeError("evaluate: more label pairs than the table can hold")
+
+    def contingency_table(self, groundtruth: "DeviceChunk", table_slots: Optional[int] = None):
+        """gala's contingency_table(seg, gt, norm=False) (reference lib/gala/evaluate.py:212-249) with nothing ignored:
+        (seg ids uint64, gt ids uint64, voxel counts uint32) host arrays, one entry per pair that occurs, sorted by (seg, gt)."""
+        work, slots, n = self._contingency(groundtruth, table_slots)
+        with self._on_device():
+            return _native.contingency_read(work.data_ptr(), slots, n, self._stream())
+
+    def evaluate_statistics(self, groundtruth: "DeviceChunk", size_thresholds=(1000,), table_slots: Optional[int] = None) -> list:
+        """One table, scored for every threshold of ``size_thresholds``: a list of dicts with the statistics (cfb_seg_scores)
+        and the five scores.  A threshold sweep costs one voxel pass."""
+        work, slots, _ = self._contingency(groundtruth, table_slots)
+        with self._on_device():
+            return [_native.contingency_scores(work.data_ptr(), slots, t, self._stream()).as_dict() for t in size_thresholds]
+
+    def evaluate(self, groundtruth: "DeviceChunk", size_threshold: float = 1000, table_slots: Optional[int] = None) -> dict:
+        """Segmentation.evaluate (reference chunk/segmentation.py:33-67) without its printed lines: rand index, adjusted rand
+        index, variation of information, Fowlkes-Mallows index and edit distance (false merges, false splits) of self against
+        ``groundtruth``, as numpy float64 like the reference's.  See include/chunkflow_b200.h for the definitions and the
+        reference quirks that are kept."""
+        st = self.evaluate_statistics(groundtruth, (size_threshold,), table_slots)[0]
+        f = np.float64
+        return {"rand_index": f(st["rand_index"]), "adjusted_rand_index": f(st["adjusted_rand_index"]),
+                "variation_of_information": f(st["variation_of_information"]),
+                "fowlkes_mallows_index": f(st["fowlkes_mallows_index"]),
+                "edit_distance": (f(st["false_merges"]), f(st["false_splits"]))}
 
     def __repr__(self):
         return f"DeviceChunk(shape={self.shape}, dtype={self.dtype}, voxel_offset={tuple(self.voxel_offset)}, device={self.tensor.device})"

@@ -135,13 +135,8 @@ __global__ void __launch_bounds__(kT) ws_merge_kernel(const uint32_t* __restrict
 
 // ---- region graph (waterz backend/region_graph.hpp + MeanAffinityProvider): one record per pair of touching fragments, the
 // sum (2^-30 fixed point: order independent) and the number of the affinities between them.  Open-addressing hash table in
-// global memory, key = (smaller id << 32 | larger id), 0 = empty slot.
-constexpr int kRgMaxProbe = 1024;
-
-__device__ __forceinline__ unsigned long long rg_hash(unsigned long long k) {
-  k ^= k >> 33; k *= 0xff51afd7ed558ccdULL; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ULL; k ^= k >> 33;
-  return k;
-}
+// global memory (hash_table.cuh), key = (smaller id << 32 | larger id), 0 = empty slot.
+#include "hash_table.cuh"
 
 __device__ __forceinline__ long long rg_quantize(float a) {
   double v = (double)a;

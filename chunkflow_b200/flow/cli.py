@@ -301,5 +301,20 @@ def agglomerate(tasks, name, input_chunk_name, output_chunk_name, threshold, aff
         yield task
 
 
+@main.command("evaluate-segmentation")
+@click.option("--segmentation-chunk-name", "-s", type=str, default="chunk", help="chunk name of segmentation")
+@click.option("--groundtruth-chunk-name", "-g", type=str, default="groundtruth")
+@click.option("--output", "-o", type=str, default="seg_score", help="segmentation evaluation result name.")
+@operator
+def evaluate_segmentation(tasks, segmentation_chunk_name, groundtruth_chunk_name, output):
+    """Evaluate segmentation by split/merge error (reference flow/flow.py:1519-1542, chunk/segmentation.py:33-67).  The
+    chunks may be host chunks (uploaded for the call) or GPU-resident ones."""
+    from chunkflow_b200.chunk.segmentation import evaluate
+    for task in tasks:
+        if task is not None:
+            task[output] = evaluate(task[segmentation_chunk_name], task[groundtruth_chunk_name])
+        yield task
+
+
 if __name__ == "__main__":
     main()

@@ -22,6 +22,8 @@
  *   cfb_device_name               Inferencer.compute_device   inferencer.py:173-175
  *   cfb_watershed_device, cfb_region_graph_*, cfb_agglomerate_edges_host, cfb_relabel_device
  *                                 plugins/agglomerate.py:8-48 (execute -> waterz.agglomerate)
+ *   cfb_contingency_*, cfb_evaluate_workspace
+ *                                 Segmentation.evaluate   chunk/segmentation.py:33-67 (-> lib/gala/evaluate.py)
  *
  * Plain pointers and sizes only -- no torch types.  Device pointers are raw CUDA device
  * addresses (e.g. torch.Tensor.data_ptr()) owned by the caller.  All functions return
@@ -73,6 +75,7 @@ extern "C" {
 #define CFB_DTYPE_U8 0
 #define CFB_DTYPE_F32 1
 #define CFB_DTYPE_U32 2 /* connected components on an integer segmentation */
+#define CFB_DTYPE_U64 3 /* segmentation evaluation: 64-bit label ids */
 
 typedef struct cfb_engine* cfb_handle;
 
@@ -294,6 +297,55 @@ int cfb_agglomerate_edges_host(int64_t num_nodes, int64_t num_edges, const uint3
 /* d_out[i] = d_map[d_labels[i]] (labels >= map_size pass through): applies root_of to the fragments. */
 int cfb_relabel_device(const uint32_t* d_labels, int64_t n, const uint32_t* d_map, int64_t map_size, uint32_t* d_out,
                        void* stream);
+
+/* `evaluate-segmentation` (DESIGN.md section 0, row f5): Segmentation.evaluate(groundtruth, size_threshold) (reference
+ * chunk/segmentation.py:33-67, called by flow/flow.py:1519-1542) scores a segmentation against ground truth with the vendored
+ * gala metrics (reference lib/gala/evaluate.py).  With c_ij the number of voxels labelled i in the segmentation and j in the
+ * ground truth (the contingency table, contingency_table :212-249):
+ *   rand / adjusted rand / Fowlkes-Mallows index  rand_values (:1183-1223) and :1248, :1274-1275, :1300, 0 an ordinary label:
+ *       a = (S1 - n) / 2, b = (S2 - S1) / 2, c = (S3 - S1) / 2, d = (S1 + n^2 - S2 - S3) / 2 with S1 = sum c^2, S2 = sum of the
+ *       squared row sums, S3 = sum of the squared column sums;
+ *   variation of information  vi -> split_vi -> vi_tables (:623-691, :1049-1101), voxels with a 0 on either side ignored:
+ *       ((xl(r') - xl(c)) + (xl(s') - xl(c))) / N', xl(v) = sum v log2 v over those voxels' table, rows r', columns s';
+ *   edit distance  raw_edit_distance (:183-209): (K - N_seg, 0.0), K = pairs with both ids != 0 and c > size_threshold,
+ *       N_seg = distinct non-zero segmentation ids.  The second element is always 0 in the reference (it slices the rows of a
+ *       1 x N matrix); kept.
+ * 0/0 gives NaN, as in the reference.  Ids are compared as the uint64 values numpy's astype(np.uint64) gives; every uint64 is
+ * a legal id (the reference itself fails on ids of about 2^40 and more; here they are scored like any other).
+ *
+ * cfb_contingency_device  d_seg, d_gt: (z,y,x) volumes of CFB_DTYPE_U8 / U32 / U64 ids (n < 2^32 voxels).  Builds the table
+ *                         of (seg id, gt id) -> count in d_workspace (cfb_evaluate_workspace(table_slots) bytes, table_slots
+ *                         a power of two below 2^31) and the statistics of all thresholds; *num_pairs = entries.  Returns
+ *                         CFB_ERR_CAPACITY when the table is too full -- call again with more slots.  Synchronises.
+ * cfb_contingency_scores  statistics + scores of the table in d_workspace for one size_threshold (compared like the
+ *                         reference's `r.data <= size_threshold`); a threshold sweep reuses the table.  Synchronises.
+ * cfb_contingency_read    the table as (seg id, gt id, count) triples sorted by (seg, gt) into host arrays of num_pairs. */
+typedef struct cfb_seg_scores {
+  int32_t struct_size;            /* = sizeof(cfb_seg_scores), for ABI checks */
+  int32_t reserved;
+  uint64_t n;                     /* voxels */
+  uint64_t sum_sq_pairs;          /* S1 */
+  uint64_t sum_sq_rows;           /* S2 */
+  uint64_t sum_sq_cols;           /* S3 */
+  uint64_t n_both_nonzero;        /* N': voxels with both ids != 0 */
+  uint64_t seg_ids;               /* N_seg: distinct non-zero segmentation ids */
+  uint64_t gt_ids;                /* N_gt: distinct non-zero ground-truth ids */
+  uint64_t pairs;                 /* entries of the contingency table */
+  uint64_t pairs_over_threshold;  /* K(size_threshold) */
+  double size_threshold;
+  double xlog_pairs;              /* xl(c) over the pairs with both ids != 0 */
+  double xlog_rows;               /* xl(r') */
+  double xlog_cols;               /* xl(s') */
+  double rand_index, adjusted_rand_index, variation_of_information, fowlkes_mallows_index;
+  double false_merges, false_splits;  /* edit distance */
+} cfb_seg_scores;
+
+int64_t cfb_evaluate_workspace(int64_t table_slots);
+int cfb_contingency_device(const void* d_seg, int32_t seg_dtype, const void* d_gt, int32_t gt_dtype, int64_t z, int64_t y,
+                           int64_t x, void* d_workspace, int64_t table_slots, int64_t* num_pairs, void* stream);
+int cfb_contingency_scores(void* d_workspace, int64_t table_slots, double size_threshold, cfb_seg_scores* out, void* stream);
+int cfb_contingency_read(void* d_workspace, int64_t table_slots, int64_t num_pairs, uint64_t* h_seg, uint64_t* h_gt,
+                         uint32_t* h_count, void* stream);
 
 #ifdef __cplusplus
 }
