@@ -33,6 +33,8 @@ EXPORTS = (
     "cfb_watershed_workspace", "cfb_watershed_device", "cfb_region_graph_workspace", "cfb_region_graph_device",
     "cfb_region_graph_read", "cfb_agglomerate_edges_host", "cfb_relabel_device",
     "cfb_evaluate_workspace", "cfb_contingency_device", "cfb_contingency_scores", "cfb_contingency_read",
+    "cfb_label_table_workspace", "cfb_label_table_device", "cfb_label_table_read", "cfb_label_table_plan",
+    "cfb_label_apply_device",
 )
 
 
@@ -148,6 +150,13 @@ def load() -> C.CDLL:
     lib.cfb_contingency_device.argtypes = [vp, i32, vp, i32, i64, i64, i64, vp, i64, C.POINTER(i64), vp]
     lib.cfb_contingency_scores.argtypes = [vp, i64, C.c_double, C.POINTER(SegScores), vp]
     lib.cfb_contingency_read.argtypes = [vp, i64, i64, vp, vp, vp, vp]
+    lib.cfb_label_table_workspace.argtypes = [i64, i64]
+    lib.cfb_label_table_workspace.restype = i64
+    lib.cfb_label_table_device.argtypes = [vp, i32, i64, i64, i64, vp, i64, C.POINTER(i64), vp]
+    lib.cfb_label_table_read.argtypes = [vp, i64, i64, vp, vp, vp, vp]
+    lib.cfb_label_table_plan.argtypes = [vp, i64, i64, i32, i64, vp, i64, i32, C.c_uint64, C.POINTER(i64), C.POINTER(i64),
+                                         C.POINTER(C.c_uint64), vp]
+    lib.cfb_label_apply_device.argtypes = [vp, i32, i64, vp, i64, vp, i32, vp]
     for name in EXPORTS:
         getattr(lib, name)   # every declared symbol must be there
     _lib = lib
@@ -282,6 +291,112 @@ def contingency_read(d_workspace: int, table_slots: int, num_pairs: int, stream:
     check(load().cfb_contingency_read(C.c_void_p(d_workspace), int(table_slots), int(num_pairs), _ptr(s), _ptr(g), _ptr(c),
                                       C.c_void_p(stream)))
     return s, g, c
+
+
+# ---- `mask-out-objects` / `remap-segmentation` (include/chunkflow_b200.h, DESIGN.md section 0, row f6) ----
+LABEL_DTYPES = (DTYPE_U8, DTYPE_U32, DTYPE_U64)
+MAX_LABEL_VOXELS = 2 ** 32 - 2
+
+
+def _label_volume(zyx) -> int:
+    """Voxel count of a (z, y, x) label volume, checked before the native side reads anything."""
+    zyx = tuple(int(v) for v in zyx)
+    if len(zyx) != 3 or min(zyx) <= 0:
+        raise ValueError(f"a label volume is (z, y, x) with positive sizes, not {zyx}")
+    n = zyx[0] * zyx[1] * zyx[2]
+    if n > MAX_LABEL_VOXELS:
+        raise ValueError("more than 2^32 - 2 voxels")
+    return n
+
+
+def _label_slots(table_slots) -> int:
+    slots = int(table_slots)
+    if slots < 32 or slots & (slots - 1) or slots >= 1 << 31:
+        raise ValueError("table_slots must be a power of two in [32, 2^31)")
+    return slots
+
+
+def _label_dtype(dtype) -> int:
+    if dtype not in LABEL_DTYPES:
+        raise TypeError("label dtype must be DTYPE_U8, DTYPE_U32 or DTYPE_U64")
+    return int(dtype)
+
+
+def check_base_id(base_id) -> int:
+    """``base_id`` of remap as a Python int in [0, 2^64 - 1]."""
+    if isinstance(base_id, bool) or not isinstance(base_id, (int, np.integer)):
+        raise TypeError(f"base_id must be an integer, not {type(base_id).__name__}")
+    base_id = int(base_id)
+    if base_id < 0:
+        raise ValueError("base_id must not be negative")
+    if base_id > 2 ** 64 - 1:
+        raise ValueError("base_id must be below 2^64")
+    return base_id
+
+
+def label_table_workspace(voxels: int, table_slots: int) -> int:
+    return int(load().cfb_label_table_workspace(int(voxels), _label_slots(table_slots)))
+
+
+def label_table_device(d_labels: int, dtype: int, zyx, d_workspace: int, table_slots: int, stream: int = 0) -> int:
+    """-> number of distinct labels; raises NativeError with code ERR_CAPACITY when the table is too small."""
+    _label_volume(zyx)
+    dtype, slots = _label_dtype(dtype), _label_slots(table_slots)
+    n = C.c_int64()
+    check(load().cfb_label_table_device(C.c_void_p(d_labels), dtype, *(int(v) for v in zyx), C.c_void_p(d_workspace), slots,
+                                        C.byref(n), C.c_void_p(stream)))
+    return int(n.value)
+
+
+def label_table_read(d_workspace: int, table_slots: int, num_labels: int, stream: int = 0):
+    """-> (ids uint64 ascending, voxel counts uint32, linear index of each id's first voxel uint32) host arrays."""
+    slots, num = _label_slots(table_slots), int(num_labels)
+    if not 0 <= num <= slots:
+        raise ValueError("num_labels must be between 0 and table_slots")
+    ids, counts, first = np.empty(num, np.uint64), np.empty(num, np.uint32), np.empty(num, np.uint32)
+    check(load().cfb_label_table_read(C.c_void_p(d_workspace), slots, num, _ptr(ids), _ptr(counts), _ptr(first), C.c_void_p(stream)))
+    return ids, counts, first
+
+
+def label_table_plan(d_workspace: int, table_slots: int, voxels: int, dust_threshold=None, d_keep_ids: int = 0, num_keep=None,
+                     renumber: bool = False, base_id: int = 0, stream: int = 0):
+    """Write every table entry's new value: 0 when ``count <= dust_threshold`` (if given) or when the id is not among the
+    ``num_keep`` ids at ``d_keep_ids`` (if ``num_keep`` is given; 0 masks everything), else the id, or with ``renumber``
+    1 + base_id + the rank of its first voxel.  -> (entries failing the dust test, surviving non-zero ids, new maximum)."""
+    slots = _label_slots(table_slots)
+    voxels = int(voxels)
+    if not 0 < voxels <= MAX_LABEL_VOXELS:
+        raise ValueError("voxels must be in [1, 2^32 - 2]")
+    base_id = check_base_id(base_id)
+    if base_id and not renumber:
+        raise ValueError("base_id needs renumber")
+    if dust_threshold is not None:
+        if isinstance(dust_threshold, bool) or not isinstance(dust_threshold, (int, np.integer)):
+            raise TypeError("the dust threshold is an integer number of voxels")
+        if not -2 ** 63 <= int(dust_threshold) < 2 ** 63:
+            raise ValueError("the dust threshold does not fit in 64 bits")
+    if num_keep is not None and (int(num_keep) < 0 or (int(num_keep) > 0 and not d_keep_ids)):
+        raise ValueError("a keep-list of num_keep >= 0 ids needs a device pointer when it is not empty")
+    dust, survivors, new_max = C.c_int64(), C.c_int64(), C.c_uint64()
+    check(load().cfb_label_table_plan(C.c_void_p(d_workspace), slots, voxels, int(dust_threshold is not None),
+                                      int(dust_threshold or 0), C.c_void_p(d_keep_ids or None), -1 if num_keep is None else int(num_keep),
+                                      int(bool(renumber)), C.c_uint64(base_id), C.byref(dust), C.byref(survivors), C.byref(new_max),
+                                      C.c_void_p(stream)))
+    return int(dust.value), int(survivors.value), int(new_max.value)
+
+
+def label_apply_device(d_in: int, in_dtype: int, voxels: int, d_workspace: int, table_slots: int, d_out: int, out_dtype: int,
+                       stream: int = 0) -> None:
+    """d_out[i] = planned new value of d_in[i]; ``d_out`` may be ``d_in`` when the dtypes are equal."""
+    in_dtype, out_dtype, slots = _label_dtype(in_dtype), _label_dtype(out_dtype), _label_slots(table_slots)
+    if out_dtype not in (in_dtype, DTYPE_U64):
+        raise TypeError("the output is of the input's dtype or uint64")
+    if d_in == d_out and in_dtype != out_dtype:
+        raise ValueError("in place needs equal dtypes")
+    if not 0 < int(voxels) <= MAX_LABEL_VOXELS:
+        raise ValueError("voxels must be in [1, 2^32 - 2]")
+    check(load().cfb_label_apply_device(C.c_void_p(d_in), in_dtype, int(voxels), C.c_void_p(d_workspace), slots, C.c_void_p(d_out),
+                                        out_dtype, C.c_void_p(stream)))
 
 
 def device_memory(device: int = 0) -> tuple:

@@ -12,6 +12,8 @@ bookkeeping of the reference's ``Chunk`` and mirrors, name for name, the referen
     connected_component  reference chunk/base.py:128-137                (Chunk -> cc3d)
     agglomerate          reference plugins/agglomerate.py:8-48          (plugin -> waterz)
     evaluate             reference chunk/segmentation.py:33-67          (Segmentation -> gala, lib/gala/evaluate.py)
+    remap, mask_fragments, mask_except
+                         reference chunk/segmentation.py:69-109         (Segmentation -> fastremap)
 
 so that ``create-chunk | normalize-contrast | inference | crop-margin | quantize`` moves the image to the GPU once and
 brings a uint8 thumbnail (or nothing) back instead of the 12-byte-per-voxel affinity map.  There is no CPU fallback.
@@ -67,6 +69,51 @@ def mask_array_for(chunk_dtype, mask: np.ndarray) -> np.ndarray:
             raise TypeError("integer mask values must be below 2**24 to be exact in float32")
         return np.ascontiguousarray(mask.astype(np.float32))
     raise TypeError(f"unsupported chunk dtype {chunk_dtype}")
+
+
+def selected_ids(selected_obj_ids) -> Optional[np.ndarray]:
+    """The id selection of Segmentation.mask_except (reference chunk/segmentation.py:92-107) as a uint64 array, or None when
+    nothing is selected: a list / set / array of ids, a string like "34,45,56", or a path ending in ``.json`` that is read as
+    a LOCAL file holding a list (the reference goes through CloudFiles; paths with a protocol are refused).  Negative ids
+    stand for their uint64 bit pattern, the repository's convention for signed label volumes."""
+    if selected_obj_ids is None:
+        return None
+    if isinstance(selected_obj_ids, np.ndarray) and selected_obj_ids.dtype.kind in "ui":
+        return np.ascontiguousarray(selected_obj_ids.ravel().astype(np.uint64))
+    if isinstance(selected_obj_ids, str) and selected_obj_ids.endswith('.json'):
+        if '://' in selected_obj_ids and not selected_obj_ids.startswith('file://'):
+            raise ValueError(f"only a local json file can hold the selected ids, not {selected_obj_ids}")
+        import json
+        with open(selected_obj_ids[len('file://'):] if selected_obj_ids.startswith('file://') else selected_obj_ids) as f:
+            selected_obj_ids = set(json.load(f))
+        assert len(selected_obj_ids) > 0                                  # reference segmentation.py:102
+        print(f'number of selected objects: {len(selected_obj_ids)}')   # :103
+    elif isinstance(selected_obj_ids, str):
+        selected_obj_ids = set(int(i) for i in selected_obj_ids.split(','))   # :107
+    ids = [int(i) for i in np.asarray(list(selected_obj_ids), dtype=object).ravel()]
+    if any(not -2 ** 63 <= i < 2 ** 64 for i in ids):
+        raise ValueError("a selected id does not fit in 64 bits")
+    return np.array([i % 2 ** 64 for i in ids], dtype=np.uint64)
+
+
+def _grown_table(device, slots: int, workspace_bytes, build, what: str):
+    """(workspace, slots, entries) of a caller-sized hash table: ``build(workspace, slots)`` returns the number of entries or
+    raises ERR_CAPACITY; the table is rebuilt four times as large while it is too full or more than half full (long probe
+    sequences)."""
+    torch = _torch()
+    while True:
+        work = torch.empty(workspace_bytes(slots), dtype=torch.uint8, device=device)
+        try:
+            n = build(work, slots)
+            if 2 * n <= slots:
+                return work, slots, n
+        except _native.NativeError as err:
+            if err.code != _native.ERR_CAPACITY:
+                raise
+        del work
+        slots <<= 2
+        if slots >= 1 << 31:
+            raise RuntimeError(f"{what} than the table can hold")
 
 
 class DeviceChunk:
@@ -258,20 +305,11 @@ class DeviceChunk:
         while slots < 16 * num_fragments:
             slots <<= 1
         with self._on_device():
-            while True:
-                work = torch.empty(_native.region_graph_workspace(slots), dtype=torch.uint8, device=t.device)
-                try:
-                    n = _native.region_graph_device(t.data_ptr(), flip_channel, f.data_ptr(), tuple(f.shape), work.data_ptr(), slots,
-                                                    self._stream())
-                    if 2 * n <= slots:
-                        break
-                except _native.NativeError as err:
-                    if err.code != _native.ERR_CAPACITY:
-                        raise
-                del work
-                slots <<= 2          # too full (or more than half full: long probe sequences): a larger table
-                if slots >= 1 << 31:
-                    raise RuntimeError("region graph: more fragment pairs than the table can hold")
+            work, slots, n = _grown_table(
+                t.device, slots, _native.region_graph_workspace,
+                lambda work, slots: _native.region_graph_device(t.data_ptr(), flip_channel, f.data_ptr(), tuple(f.shape),
+                                                                work.data_ptr(), slots, self._stream()),
+                "region graph: more fragment pairs")
             return _native.region_graph_read(work.data_ptr(), slots, n, self._stream())
 
     def agglomerate(self, threshold: float = 0.7, aff_threshold_low: float = 0.001, aff_threshold_high: float = 0.9999,
@@ -337,20 +375,11 @@ class DeviceChunk:
             raise ValueError(f"segmentation {tuple(s.shape)} and ground truth {tuple(g.shape)} must have the same shape and device")
         slots = int(table_slots) if table_slots is not None else 1 << max(10, min(24, (s.numel() // 64).bit_length()))
         with self._on_device():
-            while True:
-                work = torch.empty(_native.evaluate_workspace(slots), dtype=torch.uint8, device=s.device)
-                try:
-                    n = _native.contingency_device(s.data_ptr(), sc, g.data_ptr(), gc, tuple(s.shape), work.data_ptr(), slots,
-                                                   self._stream())
-                    if 2 * n <= slots:
-                        return work, slots, n
-                except _native.NativeError as err:
-                    if err.code != _native.ERR_CAPACITY:
-                        raise
-                del work
-                slots <<= 2          # too full (or more than half full: long probe sequences): a larger table
-                if slots >= 1 << 31:
-                    raise RuntimeError("evaluate: more label pairs than the table can hold")
+            return _grown_table(
+                s.device, slots, _native.evaluate_workspace,
+                lambda work, slots: _native.contingency_device(s.data_ptr(), sc, g.data_ptr(), gc, tuple(s.shape), work.data_ptr(),
+                                                               slots, self._stream()),
+                "evaluate: more label pairs")
 
     def contingency_table(self, groundtruth: "DeviceChunk", table_slots: Optional[int] = None):
         """gala's contingency_table(seg, gt, norm=False) (reference lib/gala/evaluate.py:212-249) with nothing ignored:
@@ -377,6 +406,89 @@ class DeviceChunk:
                 "variation_of_information": f(st["variation_of_information"]),
                 "fowlkes_mallows_index": f(st["fowlkes_mallows_index"]),
                 "edit_distance": (f(st["false_merges"]), f(st["false_splits"]))}
+
+    # ---- Segmentation.remap / mask_fragments / mask_except: label table + one relabelling pass --------------
+    def _label_table(self, table_slots: Optional[int] = None):
+        """(label tensor, dtype code, workspace, slots, labels): the table id -> (voxel count, first voxel) of the volume, built
+        on the device in one read.  The table starts at ``table_slots`` (default: from the voxel count) and is grown on
+        overflow."""
+        t, code = self._label_tensor()
+        if t.numel() == 0:
+            raise ValueError("an empty volume has no labels")
+        n = t.numel()
+        slots = int(table_slots) if table_slots is not None else 1 << max(10, min(24, (n // 64).bit_length()))
+        with self._on_device():
+            work, slots, num = _grown_table(
+                t.device, slots, lambda slots: _native.label_table_workspace(n, slots),
+                lambda work, slots: _native.label_table_device(t.data_ptr(), code, tuple(t.shape), work.data_ptr(), slots,
+                                                               self._stream()),
+                "label table: more labels")
+        return t, code, work, slots, num
+
+    def _label_numpy_dtype(self, code):
+        return {_native.DTYPE_U8: np.uint8, _native.DTYPE_U32: np.uint32, _native.DTYPE_U64: np.uint64}[code]
+
+    def unique(self, return_counts: bool = False, table_slots: Optional[int] = None):
+        """fastremap.unique of the label volume (as the reference uses it, chunk/segmentation.py:87): the ids in ascending
+        order (as unsigned values, in the volume's unsigned dtype) and, with ``return_counts``, their voxel counts (int64).
+        One read of the volume; only the table comes to the host."""
+        _, code, work, slots, num = self._label_table(table_slots)
+        with self._on_device():
+            ids, counts, _ = _native.label_table_read(work.data_ptr(), slots, num, self._stream())
+        ids = ids.astype(self._label_numpy_dtype(code))
+        return (ids, counts.astype(np.int64)) if return_counts else ids
+
+    def _relabel(self, dust_threshold=None, keep_ids: Optional[np.ndarray] = None, renumber: bool = False, base_id: int = 0,
+                 table_slots: Optional[int] = None):
+        """Count pass, plan and apply pass (csrc/relabel.cu); the tensor is replaced by the result.  Masks keep the dtype and
+        work in place; renumbering gives the uint64 bit pattern in an int64 tensor.
+        -> (labels in the volume, entries failing the dust test, surviving non-zero ids, maximum of the result)."""
+        torch = _torch()
+        base_id = _native.check_base_id(base_id)
+        t, code, work, slots, num = self._label_table(table_slots)
+        shape = tuple(self.tensor.shape)
+        with self._on_device():
+            d_keep = None
+            if keep_ids is not None and keep_ids.size:
+                d_keep = torch.from_numpy(np.ascontiguousarray(keep_ids, np.uint64).view(np.int64)).to(t.device)
+            dust, survivors, new_max = _native.label_table_plan(
+                work.data_ptr(), slots, t.numel(), dust_threshold, d_keep.data_ptr() if d_keep is not None else 0,
+                None if keep_ids is None else int(keep_ids.size), renumber, base_id, self._stream())
+            out = torch.empty(t.shape, dtype=torch.int64, device=t.device) if renumber else t
+            _native.label_apply_device(t.data_ptr(), code, t.numel(), work.data_ptr(), slots, out.data_ptr(),
+                                       _native.DTYPE_U64 if renumber else code, self._stream())   # synchronises: d_keep may go
+        self.tensor = out.view(shape)
+        self.layer_type = "segmentation"
+        return num, dust, survivors, new_max
+
+    def mask_out_objects(self, dust_size_threshold: Optional[int] = None, selected_obj_ids=None,
+                         table_slots: Optional[int] = None) -> tuple:
+        """mask_fragments and then mask_except (the order of `mask-out-objects`, reference flow/flow.py:2044-2047) sharing one
+        count pass and one relabelling pass; either may be None.  In place.  -> (labels in the volume, labels failing the dust
+        test): the two numbers mask_fragments prints."""
+        keep = selected_ids(selected_obj_ids)
+        if dust_size_threshold is None and keep is None:
+            return None
+        num, dust, _, _ = self._relabel(dust_threshold=dust_size_threshold, keep_ids=keep, table_slots=table_slots)
+        return num, dust
+
+    def mask_fragments(self, voxel_num_threshold: int, table_slots: Optional[int] = None) -> tuple:
+        """Segmentation.mask_fragments (reference chunk/segmentation.py:86-90) without its printed line: every id with
+        ``count <= voxel_num_threshold`` becomes 0 (`<=`, like the reference's code).  In place, dtype unchanged.
+        -> (labels in the volume, labels masked), 0 counted in both like the reference's line."""
+        return self.mask_out_objects(dust_size_threshold=int(voxel_num_threshold), table_slots=table_slots)
+
+    def mask_except(self, selected_obj_ids, table_slots: Optional[int] = None) -> None:
+        """Segmentation.mask_except (reference chunk/segmentation.py:92-109): every id not selected becomes 0; ids that do not
+        occur are ignored; an empty selection gives an all-zero volume; None does nothing.  In place, dtype unchanged."""
+        self.mask_out_objects(selected_obj_ids=selected_obj_ids, table_slots=table_slots)
+
+    def remap(self, base_id: int = 0, table_slots: Optional[int] = None) -> int:
+        """Segmentation.remap (reference chunk/segmentation.py:69-84): the non-zero ids become 1..N in the order in which they
+        are first met in a C-order raster scan (fastremap.renumber, preserve_zero=True), plus ``base_id``; 0 stays 0.  The
+        tensor becomes the uint64 result (bit pattern in an int64 tensor).  Returns the maximum of the result, the base id of
+        the next chunk -- 0 for an all-zero chunk whatever ``base_id``: the reference's value, kept."""
+        return self._relabel(renumber=True, base_id=base_id, table_slots=table_slots)[3]
 
     def __repr__(self):
         return f"DeviceChunk(shape={self.shape}, dtype={self.dtype}, voxel_offset={tuple(self.voxel_offset)}, device={self.tensor.device})"

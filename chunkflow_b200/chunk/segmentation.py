@@ -1,7 +1,8 @@
-"""A segmentation chunk (reference chunk/segmentation.py:17-67): ``Segmentation.evaluate`` scores it against ground truth.
+"""A segmentation chunk (reference chunk/segmentation.py:17-109): ``Segmentation.evaluate`` scores it against ground truth,
+``remap`` renumbers its ids, ``mask_fragments`` and ``mask_except`` remove dust and unselected objects.
 
-The scores are computed on the GPU (``DeviceChunk.evaluate``, csrc/evaluate.cu): host chunks are uploaded for the call.
-There is no CPU fallback.
+Everything is computed on the GPU (``DeviceChunk.evaluate``, csrc/evaluate.cu; ``DeviceChunk.remap`` / ``mask_out_objects``,
+csrc/relabel.cu): host chunks are uploaded for the call and the result is downloaded.  There is no CPU fallback.
 """
 from __future__ import annotations
 
@@ -64,6 +65,33 @@ class Segmentation(Chunk):
         """
         return evaluate(self, groundtruth, size_threshold, device)
 
+    def remap(self, base_id: int = 0, device="cuda:0"):
+        """renumber the object ID (reference chunk/segmentation.py:69-84)
+
+        Args:
+            base_id (int, optional): the maximum object ID in previous chunk. Defaults to 0.
+
+        Returns:
+            new_base_id (int): the maximum object ID in this chunk as the new base ID (0 for an all-zero chunk, whatever
+            ``base_id``, like the reference).  ``self.array`` becomes uint64.
+        """
+        dev = _device_labels(self, device)
+        new_base_id = dev.remap(base_id)
+        self.array = dev.tensor.cpu().numpy().view(np.uint64)
+        return np.uint64(new_base_id)
+
+    def mask_fragments(self, voxel_num_threshold: int, device="cuda:0"):
+        """Ids with ``voxel count <= voxel_num_threshold`` become 0 (reference chunk/segmentation.py:86-90)."""
+        mask_out_objects(self, dust_size_threshold=voxel_num_threshold, device=device)
+
+    def mask_except(self, selected_obj_ids, device="cuda:0"):
+        """Ids outside ``selected_obj_ids`` (a list, a set, "34,45,56" or a local .json file) become 0 (reference
+        chunk/segmentation.py:92-109)."""
+        if selected_obj_ids is None:
+            print('we have not selected any objects to mask out.')
+            return
+        mask_out_objects(self, selected_obj_ids=selected_obj_ids, device=device)
+
 
 def evaluate(segmentation, groundtruth, size_threshold: int = 1000, device="cuda:0") -> dict:
     """Segmentation.evaluate for any mix of host chunks, arrays and DeviceChunks (a DeviceChunk segmentation keeps its GPU);
@@ -73,3 +101,28 @@ def evaluate(segmentation, groundtruth, size_threshold: int = 1000, device="cuda
     ret = seg.evaluate(gt, size_threshold=size_threshold)
     print(report(ret), end="")
     return ret
+
+
+def _host_labels(dev, dtype) -> np.ndarray:
+    """The labels of a DeviceChunk made by _device_labels, back in the host dtype they came from."""
+    arr = dev.tensor.cpu().numpy()
+    if arr.dtype == np.int32:
+        return arr.view(np.uint32).astype(dtype, copy=False)
+    if arr.dtype == np.int64:
+        return arr.view(np.uint64).astype(dtype, copy=False)   # masked values are 0 or unchanged: they fit
+    return arr.astype(dtype, copy=False)
+
+
+def mask_out_objects(segmentation, dust_size_threshold=None, selected_obj_ids=None, device="cuda:0"):
+    """``mask_fragments`` and then ``mask_except`` (the body of `mask-out-objects`, reference flow/flow.py:2044-2047) with
+    one count pass and one relabelling pass on the GPU for both; prints the line mask_fragments prints.  A DeviceChunk is
+    changed in place and stays on its GPU; a host chunk gets a new ``array`` of the same dtype.  Returns ``segmentation``."""
+    from .device import DeviceChunk
+    dev = _device_labels(segmentation, device)
+    report = dev.mask_out_objects(dust_size_threshold, selected_obj_ids)
+    if report is not None and dust_size_threshold is not None:
+        num, dust = report
+        print(f'masking out {dust} fragments in {num} with a percentage of {dust / num}')   # reference segmentation.py:89
+    if report is not None and not isinstance(segmentation, DeviceChunk):
+        segmentation.array = _host_labels(dev, segmentation.array.dtype)
+    return segmentation

@@ -316,5 +316,55 @@ def evaluate_segmentation(tasks, segmentation_chunk_name, groundtruth_chunk_name
         yield task
 
 
+@main.command("mask-out-objects")
+@click.option("--input-chunk-name", "-i", type=str, default="chunk")
+@click.option("--output_chunk_name", "-o", type=str, default="chunk")
+@click.option("--dust-size-threshold", "-d", type=click.INT, default=None,
+              help="eliminate small objects with voxel number less than or equal to threshold.")
+@click.option("--selected-obj-ids", "-s", type=str, default=None,
+              help="a list of segment ids to keep. This is for sparse meshing. The ids should be separated by comma without "
+                   "space, such as \"34,56,78,90\"; it can also be a local json file that contains a list of ids.")
+@operator
+def mask_out_objects(tasks, input_chunk_name, output_chunk_name, dust_size_threshold, selected_obj_ids):
+    """Mask out objects in a segmentation chunk (reference flow/flow.py:2015-2050): dust first, then everything outside the
+    selection, in one pass over the table of labels and one over the volume.  A host chunk gives a host Segmentation, a
+    GPU-resident chunk is changed where it is."""
+    from chunkflow_b200.chunk.device import DeviceChunk, selected_ids
+    from chunkflow_b200.chunk.segmentation import Segmentation, mask_out_objects as run
+    if selected_obj_ids is not None:
+        selected_obj_ids = selected_ids(selected_obj_ids)   # parsed (and a json file read) once, like the reference
+    for task in tasks:
+        if task is not None:
+            seg = task[input_chunk_name]
+            if not isinstance(seg, (Segmentation, DeviceChunk)):
+                assert isinstance(seg, Chunk)
+                seg = Segmentation.from_chunk(seg)
+            task[output_chunk_name] = run(seg, dust_size_threshold, selected_obj_ids)
+        yield task
+
+
+@main.command("remap-segmentation")
+@click.option("--input-chunk-name", "-i", type=str, default="chunk", help="input chunk name")
+@click.option("--output-chunk-name", "-o", type=str, default="chunk", help="output chunk name")
+@click.option("--base-id", type=click.INT, default=None,
+              help="the ids start after this one (default: the task's base_id, the largest id of the previous remap, or 0).")
+@operator
+def remap_segmentation(tasks, input_chunk_name, output_chunk_name, base_id):
+    """(extension) Renumber the object ids to 1..N in raster order of their first voxel, after --base-id (reference
+    chunk/segmentation.py:69-84; the reference has the method but no command).  The largest new id is stored in
+    task['base_id'], where the next remap of the same invocation starts, so that its chunks get disjoint id ranges."""
+    from chunkflow_b200.chunk.device import DeviceChunk
+    from chunkflow_b200.chunk.segmentation import Segmentation
+    for task in tasks:
+        if task is not None:
+            seg = task[input_chunk_name]
+            if not isinstance(seg, (Segmentation, DeviceChunk)):
+                assert isinstance(seg, Chunk)
+                seg = Segmentation.from_chunk(seg)
+            task["base_id"] = int(seg.remap(task.get("base_id", 0) if base_id is None else base_id))
+            task[output_chunk_name] = seg
+        yield task
+
+
 if __name__ == "__main__":
     main()

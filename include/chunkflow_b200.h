@@ -24,6 +24,8 @@
  *                                 plugins/agglomerate.py:8-48 (execute -> waterz.agglomerate)
  *   cfb_contingency_*, cfb_evaluate_workspace
  *                                 Segmentation.evaluate   chunk/segmentation.py:33-67 (-> lib/gala/evaluate.py)
+ *   cfb_label_table_*, cfb_label_apply_device
+ *                                 Segmentation.remap / mask_fragments / mask_except   chunk/segmentation.py:69-109
  *
  * Plain pointers and sizes only -- no torch types.  Device pointers are raw CUDA device
  * addresses (e.g. torch.Tensor.data_ptr()) owned by the caller.  All functions return
@@ -75,7 +77,7 @@ extern "C" {
 #define CFB_DTYPE_U8 0
 #define CFB_DTYPE_F32 1
 #define CFB_DTYPE_U32 2 /* connected components on an integer segmentation */
-#define CFB_DTYPE_U64 3 /* segmentation evaluation: 64-bit label ids */
+#define CFB_DTYPE_U64 3 /* segmentation evaluation and clean-up: 64-bit label ids */
 
 typedef struct cfb_engine* cfb_handle;
 
@@ -346,6 +348,42 @@ int cfb_contingency_device(const void* d_seg, int32_t seg_dtype, const void* d_g
 int cfb_contingency_scores(void* d_workspace, int64_t table_slots, double size_threshold, cfb_seg_scores* out, void* stream);
 int cfb_contingency_read(void* d_workspace, int64_t table_slots, int64_t num_pairs, uint64_t* h_seg, uint64_t* h_gt,
                          uint32_t* h_count, void* stream);
+
+/* Segmentation clean-up (DESIGN.md section 0, row f6): Segmentation.mask_fragments(t) / mask_except(ids) / remap(base_id)
+ * (reference chunk/segmentation.py:69-109; the first two are the `mask-out-objects` command, flow/flow.py:2015-2050).  The
+ * reference delegates to fastremap (unique, mask, mask_except, renumber), a third-party package outside the reference tree:
+ * its behaviour is restated (oracle/relabel_oracle.py), the reference's own code around it is pinned by golden vectors.
+ *   dust       every id whose voxel count is <= t becomes 0 (`<=`, as the reference's code has it, not its help text);
+ *   keep-list  every id that is not listed becomes 0; listed ids that do not occur are ignored; an empty list masks all;
+ *   renumber   the surviving non-zero ids become 1..N in the order of their first voxels in a C-order raster scan, plus
+ *              base_id; 0 stays 0; the output is uint64.  Masking never reorders first voxels, so the three compose.
+ * Every uint64 is a legal id.  Volumes hold at most 2^32 - 2 voxels (first-voxel indices are 32-bit) and are 16-byte aligned.
+ *
+ * cfb_label_table_workspace  bytes of d_workspace for a volume of `voxels` and a table of table_slots (a power of two in
+ *                            [32, 2^31)).
+ * cfb_label_table_device     one read of the (z,y,x) volume of CFB_DTYPE_U8 / U32 / U64 ids builds
+ *                            id -> (voxel count, linear index of the first voxel) in d_workspace; *num_labels = entries (0
+ *                            included when it occurs).  CFB_ERR_CAPACITY when the table is too full -- call again with more
+ *                            slots.  Synchronises.
+ * cfb_label_table_read       the table as host arrays of num_labels, ids ascending.
+ * cfb_label_table_plan       writes every entry's new value for any combination of use_dust (count <= dust_threshold),
+ *                            a keep-list of num_keep ids in device memory (num_keep < 0: none) and renumber (+ base_id;
+ *                            base_id + N > 2^64 - 1 is refused).  *num_dust = entries failing the dust test (0 included: the
+ *                            first number mask_fragments prints), *num_survivors = non-zero ids that stay non-zero, *new_max =
+ *                            the maximum of the relabelled volume (0 when nothing survives, whatever base_id: the value the
+ *                            reference returns).  No voxel is read.  Synchronises.
+ * cfb_label_apply_device     second read of the volume, one write: d_out[i] = new value of d_in[i].  out_dtype is in_dtype
+ *                            (d_out may then be d_in) or CFB_DTYPE_U64, which a renumbering plan requires.  Synchronises. */
+int64_t cfb_label_table_workspace(int64_t voxels, int64_t table_slots);
+int cfb_label_table_device(const void* d_labels, int32_t dtype, int64_t z, int64_t y, int64_t x, void* d_workspace,
+                           int64_t table_slots, int64_t* num_labels, void* stream);
+int cfb_label_table_read(void* d_workspace, int64_t table_slots, int64_t num_labels, uint64_t* h_ids, uint32_t* h_counts,
+                         uint32_t* h_first, void* stream);
+int cfb_label_table_plan(void* d_workspace, int64_t table_slots, int64_t voxels, int32_t use_dust, int64_t dust_threshold,
+                         const uint64_t* d_keep_ids, int64_t num_keep, int32_t renumber, uint64_t base_id, int64_t* num_dust,
+                         int64_t* num_survivors, uint64_t* new_max, void* stream);
+int cfb_label_apply_device(const void* d_in, int32_t in_dtype, int64_t voxels, void* d_workspace, int64_t table_slots,
+                           void* d_out, int32_t out_dtype, void* stream);
 
 #ifdef __cplusplus
 }
