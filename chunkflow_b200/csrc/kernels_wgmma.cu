@@ -4,7 +4,7 @@
 //
 //   warp 0       : A producer  -- one TMA box per z-plane (halo rows/cols, zero fill outside the patch)
 //   warp 1       : B producer  -- the packed weights of one tap per stage via cp.async.bulk
-//   warpgroups 1, 2: consumers -- per z-plane job: 27 taps x K steps x MT tiles of wgmma.mma_async
+//   warpgroups 1, 2: consumers -- per z-plane job: 27 taps x K steps x (up to MT) tiles of wgmma.mma_async
 //                                 (M = 64 positions, N = Cout or 2 * Cout, fp32 accumulators in registers),
 //                                 then the epilogue: bias, ReLU, number format, 16-byte stores
 //
@@ -24,6 +24,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "act_format.cuh"
@@ -63,16 +64,13 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
   return ok != 0;
 }
 // Bounded wait: a protocol bug becomes a launch failure (trap) instead of a hung GPU.  The bound (~1 min at 2 GHz) is far
-// beyond any legitimate wait, including time-slicing with other contexts on a shared GPU.
+// beyond any legitimate wait, including time-slicing with other contexts on a shared GPU.  No printf here: a function call
+// anywhere in the kernel makes ptxas serialize every wgmma of it (C7510).
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 120000000000ll) {
-      printf("chunkflow_b200: mbarrier timeout (block %d thread %d bar 0x%x parity %u)\n", (int)blockIdx.x,
-             (int)threadIdx.x, bar, parity);
-      __trap();
-    }
+    if (clock64() - t0 > 120000000000ll) __trap();
   }
 }
 __device__ __forceinline__ bool elect_one() {
@@ -287,6 +285,17 @@ __host__ __device__ constexpr int stage_bytes() {
   return (MODE == kConvPool ? kConsumers * Cfg::MT : kConsumers) * 64 * Cfg::SP * 4;
 }
 
+// Calls f(std::integral_constant<int, n>) for a runtime n in [0, N]: a count the compiler must see as a constant.
+template <int N, typename F>
+__device__ __forceinline__ void with_tile_count(int n, F&& f) {
+  if constexpr (N == 0) {
+    f(std::integral_constant<int, 0>{});
+  } else {
+    if (n == N) f(std::integral_constant<int, N>{});
+    else with_tile_count<N - 1>(n, f);
+  }
+}
+
 template <int CIN, int COUT, int FMT, bool TAIL, int MODE>
 __global__ void __launch_bounds__(kThreads, 1)
 conv3_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
@@ -370,8 +379,8 @@ conv3_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
   const int cw = (warp >> 2) - 1;           // consumer warpgroup 0 / 1
   const int wtid = threadIdx.x & 127;       // thread in the warpgroup
   const bool leader = wtid == 0;
-  const int g0 = cw * MT;                   // first M tile of this warpgroup
-  const int ntiles = max(0, min(MT, p.G - g0));
+  const int n0 = (p.G + 1) >> 1;            // the G tiles of the CTA, split evenly: ceil(G / 2) <= MT to warpgroup 0
+  const int g0 = cw ? n0 : 0;               // first M tile of this warpgroup
   const uint32_t sA0 = smem_u32(sA), sB0 = smem_u32(sB);
   const uint32_t pitch = (uint32_t)p.pitch;
   const uint32_t a_lbo = (uint32_t)P * p.plane_stride;  // chunk 2k -> chunk 2k + 1 of a K step
@@ -380,191 +389,188 @@ conv3_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
   float* stage = s_stage + (MODE == kConvPool ? 0 : (size_t)cw * 64 * Cfg::SP);
   const int ty_valid = min(p.TY, p.Y - y0), xt_valid = min(p.XT, p.X - x0);
   const size_t plane_vox = (size_t)p.Z * p.Y * p.X;
-  uint4* out16 = reinterpret_cast<uint4*>(p.out);
+  // this batch entry's planes of the output (and of the pooled output): per-voxel addresses need no 64-bit products
+  uint4* out16 = reinterpret_cast<uint4*>(p.out) + (size_t)b * (COUT / 8) * P * (MODE == kConvT ? 4 : 1) * plane_vox;
+  uint4* pool16 = MODE == kConvPool ? reinterpret_cast<uint4*>(p.out_pool) + (size_t)b * (COUT / 8) * P * (plane_vox / 4) : nullptr;
 
-  float acc[MT][NA / 2];
-  uint32_t ring_st = 0, ring_parity = 0;
-  for (int zz = 0; zz < Z; ++zz) {
-    const int z = z0 + zz;
+  // The consumer body is instantiated per tile count NTL.  A wgmma behind a runtime tile guard sits on a path the compiler
+  // treats as divergent, and ptxas then serializes every wgmma of the kernel (a full wait after each product).
+  with_tile_count<MT>(cw ? p.G - n0 : n0, [&](auto tiles) {
+    constexpr int NTL = decltype(tiles)::value;  // M tiles of this warpgroup
+    float acc[NTL > 0 ? NTL : 1][NA / 2];
+    uint32_t ring_st = 0, ring_parity = 0;
+    for (int zz = 0; zz < Z; ++zz) {
+      const int z = z0 + zz;
+      int prev_st = -1;
+      // ---------------- epilogue: registers -> staging tile -> bias/ReLU -> number format -> HBM ----------------
+      // accumulator fragment of m64nN: thread (warp w, lane l) holds rows 16 w + l / 4 (+ 8), columns 8 j + 2 (l % 4) (+ 1)
+      auto epilogue = [&](int par) {
+        wg_wait<0>();
 #pragma unroll
-    for (int g = 0; g < MT; ++g)
+        for (int g = 0; g < NTL; ++g) acc_fence(acc[g]);
+        if (leader && prev_st >= 0) mbar_arrive(BAR(kBE + prev_st));  // the job's last weight stage
+        prev_st = -1;
+        const int wr = (wtid >> 5) * 16 + ((wtid & 31) >> 2), wc = 2 * (wtid & 3);
+        // one voxel's 16 channels from the staging rows: accumulator scale, bias, ReLU
+        auto load16 = [&](int row, int cb, float (&v)[16]) {
+          const float4* src = reinterpret_cast<const float4*>(stage + row * Cfg::SP + cb * 16);
 #pragma unroll
-      for (int i = 0; i < NA / 2; ++i) acc[g][i] = 0.f;
-    int prev_st = -1;
-    // ---------------- epilogue: registers -> staging tile -> bias/ReLU -> number format -> HBM ----------------
-    // accumulator fragment of m64nN: thread (warp w, lane l) holds rows 16 w + l / 4 (+ 8), columns 8 j + 2 (l % 4) (+ 1)
-    auto epilogue = [&](int par) {
-      wg_wait<0>();
+          for (int i = 0; i < 4; ++i) {
+            const float4 f = src[i];
+            v[4 * i] = f.x; v[4 * i + 1] = f.y; v[4 * i + 2] = f.z; v[4 * i + 3] = f.w;
+          }
 #pragma unroll
-      for (int g = 0; g < MT; ++g) acc_fence(acc[g]);
-      if (leader && prev_st >= 0) mbar_arrive(BAR(kBE + prev_st));  // the job's last weight stage
-      prev_st = -1;
-      if (MODE != kConvT && leader) mbar_arrive(BAR(kAE + (zz % kRing)));  // plane z-1 is dead: the producer may refill its slot
-      const int wr = (wtid >> 5) * 16 + ((wtid & 31) >> 2), wc = 2 * (wtid & 3);
-      // one voxel's 16 channels from the staging rows: accumulator scale, bias, ReLU
-      auto load16 = [&](int row, int cb, float (&v)[16]) {
-        const float4* src = reinterpret_cast<const float4*>(stage + row * Cfg::SP + cb * 16);
+          for (int i = 0; i < 16; ++i) {
+            v[i] = fmaf(v[i], p.acc_scale, __ldg(p.bias + cb * 16 + i));
+            if (p.relu) v[i] = relu_nan(v[i]);
+          }
+        };
+        auto store16 = [&](const float (&v)[16], int cb, size_t vox, size_t pvol, uint4* dst) {
+          if constexpr (FMT == kFmtF16F8) store_cp8_16_f8<COUT>(v, cb, 0, vox, pvol, dst);
+          else store_cp8_16<COUT, FMT == kFmtF16x2>(v, cb, 0, vox, pvol, dst);
+        };
+        // kConvPool stages every tile of the CTA (rows = CTA positions) before anyone reads; otherwise one tile at a time
+        constexpr int NPASS = MODE == kConvPool ? 1 : NTL;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float4 f = src[i];
-          v[4 * i] = f.x; v[4 * i + 1] = f.y; v[4 * i + 2] = f.z; v[4 * i + 3] = f.w;
-        }
+        for (int pass = 0; pass < NPASS; ++pass) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          v[i] = fmaf(v[i], p.acc_scale, __ldg(p.bias + cb * 16 + i));
-          if (p.relu) v[i] = relu_nan(v[i]);
+          for (int g = 0; g < NTL; ++g) {
+            if (MODE != kConvPool && g != pass) continue;
+            const int row0 = MODE == kConvPool ? (g0 + g) * 64 : 0;
+#pragma unroll
+            for (int j = 0; j < COUT / 8; ++j) {
+              float v0 = acc[g][4 * j], v1 = acc[g][4 * j + 1], v2 = acc[g][4 * j + 2], v3 = acc[g][4 * j + 3];
+              if constexpr (FMT != kFmtF16) {  // + the second half (f16x2: w_lo columns of the first product; f16f8: e4m3 product)
+                v0 += acc[g][COUT / 2 + 4 * j]; v1 += acc[g][COUT / 2 + 4 * j + 1];
+                v2 += acc[g][COUT / 2 + 4 * j + 2]; v3 += acc[g][COUT / 2 + 4 * j + 3];
+              }
+              *reinterpret_cast<float2*>(stage + (row0 + wr) * Cfg::SP + 8 * j + wc) = make_float2(v0, v1);
+              *reinterpret_cast<float2*>(stage + (row0 + wr + 8) * Cfg::SP + 8 * j + wc) = make_float2(v2, v3);
+            }
+          }
+          if (MODE == kConvPool) named_sync(3, 256); else named_sync(1 + cw, 128);
+          // rows handled by this pass and the threads sharing them
+          const int nrows = MODE == kConvPool ? p.G * 64 : 64, tid = MODE == kConvPool ? (int)threadIdx.x - 128 : wtid;
+          const int nthr = MODE == kConvPool ? 256 : 128, rowq0 = MODE == kConvPool ? 0 : (g0 + pass) * 64;
+#pragma unroll
+          for (int cb = 0; cb < COUT / 16; ++cb)
+          for (int row = tid; row < nrows; row += nthr) {
+            const int qpos = rowq0 + row;
+            const int r = qpos / p.pitch, col = qpos - r * p.pitch;
+            if (r >= ty_valid || col >= xt_valid) continue;
+            float v[16];
+            load16(row, cb, v);
+            if constexpr (MODE == kConvT) {  // output parity par = (oy & 1) * 2 + (ox & 1) on the doubled grid
+              const int oy = 2 * (y0 + r) + (par >> 1), ox = 2 * (x0 + col) + (par & 1);
+              store16(v, cb, ((size_t)z * 2 * p.Y + oy) * 2 * p.X + ox, plane_vox * 4, out16);
+            } else if constexpr (TAIL) {
+              head_blend_16(v, p.tail, s_head, pp, z, y0 + r, x0 + col);
+            } else {
+              store16(v, cb, ((size_t)z * p.Y + (y0 + r)) * p.X + (x0 + col), plane_vox, out16);
+            }
+          }
+          if constexpr (MODE == kConvPool) {  // (1,2,2) max pool of the same values (y0, x0, TY, XT and the extents are even)
+            const int PX = p.XT / 2, npool = (p.TY / 2) * PX;
+#pragma unroll
+            for (int cb = 0; cb < COUT / 16; ++cb)
+            for (int pi = tid; pi < npool; pi += nthr) {
+              const int pr = pi / PX, pc = pi - pr * PX;
+              if (2 * pr >= ty_valid || 2 * pc >= xt_valid) continue;
+              float m[16], v[16];
+#pragma unroll
+              for (int i = 0; i < 16; ++i) m[i] = -INFINITY;
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                load16((2 * pr + (k >> 1)) * p.pitch + 2 * pc + (k & 1), cb, v);
+#pragma unroll
+                for (int i = 0; i < 16; ++i) m[i] = fmaxf(m[i], v[i]);
+              }
+              const size_t pvox = ((size_t)z * (p.Y / 2) + (y0 / 2 + pr)) * (p.X / 2) + (x0 / 2 + pc);
+              store16(m, cb, pvox, plane_vox / 4, pool16);
+            }
+          }
+          if (MODE == kConvPool) named_sync(3, 256); else named_sync(1 + cw, 128);
         }
       };
-      auto store16 = [&](const float (&v)[16], int cb, size_t vox, size_t pvol, uint4* dst) {
-        if constexpr (FMT == kFmtF16F8) store_cp8_16_f8<COUT>(v, cb, b, vox, pvol, dst);
-        else store_cp8_16<COUT, FMT == kFmtF16x2>(v, cb, b, vox, pvol, dst);
-      };
-      // kConvPool stages every tile of the CTA (rows = CTA positions) before anyone reads; otherwise one tile at a time
-      constexpr int NPASS = MODE == kConvPool ? 1 : MT;
-      for (int pass = 0; pass < NPASS; ++pass) {
-        if (MODE != kConvPool && pass >= ntiles) break;
+      if (MODE == kConvT && zz == 0) mbar_wait(BAR(kAF + 0), 0);  // plane z0 - 1 (unused) must have landed before its slot is freed
+      // conv: 27 taps accumulate into one job; convT: the 4 output parities are 4 jobs on the centre tap of plane z.
+      // Barrier waits and arrivals stay outside the span from wgmma.fence to commit_group.
+      for (int t = 0; t < NT; ++t) {
+        const int dz = MODE == kConvT ? 1 : t / 9, dy = MODE == kConvT ? 1 : (t / 3) % 3, dx = MODE == kConvT ? 1 : t % 3;
+        const int q = zz + dz, slot = q % kRing;
+        if (MODE == kConvT ? t == 0 : (dy == 0 && dx == 0)) mbar_wait(BAR(kAF + slot), (uint32_t)(q / kRing) & 1u);
+        const uint32_t a_slot = sA0 + (uint32_t)slot * p.slot_stride;
+        // the job's first products overwrite the accumulators (scale-d = 0): zeroing them with register moves makes ptxas
+        // serialize every wgmma of the kernel (C7518)
+        const int first = MODE == kConvT || t == 0;
+        uint32_t st;
+        if (resident) {
+          st = (uint32_t)t;
+          if (zz == 0) mbar_wait(BAR(kBF + st), 0);  // taps arrive once
+        } else {
+          st = ring_st;
+          mbar_wait(BAR(kBF + st), ring_parity);
+          if (++ring_st == nbs) { ring_st = 0; ring_parity ^= 1; }
+        }
+        const uint32_t b_tap = sB0 + st * Cfg::TAP;
+        const uint32_t a_tap = a_slot + (uint32_t)(dy * pitch + dx) * 16u;
 #pragma unroll
-        for (int g = 0; g < MT; ++g) {
-          if (MODE == kConvPool ? g >= ntiles : g != pass) continue;
-          const int row0 = MODE == kConvPool ? (g0 + g) * 64 : 0;
+        for (int g = 0; g < NTL; ++g) acc_fence(acc[g]);
+        wg_fence();
+        // main products; accumulator accesses are ordered only between wgmma of the same shape, so the f16x2 second
+        // products (same registers, different shape) wait for the first group; the f16f8 e4m3 products use their own half
 #pragma unroll
-          for (int j = 0; j < COUT / 8; ++j) {
-            float v0 = acc[g][4 * j], v1 = acc[g][4 * j + 1], v2 = acc[g][4 * j + 2], v3 = acc[g][4 * j + 3];
-            if constexpr (FMT != kFmtF16) {  // + the second half (f16x2: w_lo columns of the first product; f16f8: e4m3 product)
-              v0 += acc[g][COUT / 2 + 4 * j]; v1 += acc[g][COUT / 2 + 4 * j + 1];
-              v2 += acc[g][COUT / 2 + 4 * j + 2]; v3 += acc[g][COUT / 2 + 4 * j + 3];
-            }
-            *reinterpret_cast<float2*>(stage + (row0 + wr) * Cfg::SP + 8 * j + wc) = make_float2(v0, v1);
-            *reinterpret_cast<float2*>(stage + (row0 + wr + 8) * Cfg::SP + 8 * j + wc) = make_float2(v2, v3);
+        for (int ks = 0; ks < Cfg::KS; ++ks) {
+          const uint32_t b_blk = b_tap + (uint32_t)ks * Cfg::BLK;
+          const uint32_t a_ks = a_tap + (uint32_t)(2 * ks * P) * p.plane_stride;
+#pragma unroll
+          for (int g = 0; g < NTL; ++g) {
+            const uint32_t a = a_ks + (uint32_t)((g0 + g) * 64) * 16u;
+            const int scd = ks == 0 && first ? 0 : 1;
+            if constexpr (FMT == kFmtF16x2) wgmma_f16<2 * COUT>(acc[g], gdesc(a, a_lbo), gdesc(b_blk, 2 * COUT * 16), scd);
+            else wgmma_f16<COUT>(reinterpret_cast<float(&)[COUT / 2]>(acc[g]), gdesc(a, a_lbo), gdesc(b_blk, COUT * 16), scd);
           }
         }
-        if (MODE == kConvPool) named_sync(3, 256); else named_sync(1 + cw, 128);
-        // rows handled by this pass and the threads sharing them
-        const int nrows = MODE == kConvPool ? p.G * 64 : 64, tid = MODE == kConvPool ? (int)threadIdx.x - 128 : wtid;
-        const int nthr = MODE == kConvPool ? 256 : 128, rowq0 = MODE == kConvPool ? 0 : (g0 + pass) * 64;
-        for (int item = tid; item < nrows * (COUT / 16); item += nthr) {
-          const int row = item % nrows, cb = item / nrows;
-          const int qpos = rowq0 + row;
-          const int r = qpos / p.pitch, col = qpos - r * p.pitch;
-          if (r >= ty_valid || col >= xt_valid) continue;
-          float v[16];
-          load16(row, cb, v);
-          if constexpr (MODE == kConvT) {  // output parity par = (oy & 1) * 2 + (ox & 1) on the doubled grid
-            const int oy = 2 * (y0 + r) + (par >> 1), ox = 2 * (x0 + col) + (par & 1);
-            store16(v, cb, ((size_t)z * 2 * p.Y + oy) * 2 * p.X + ox, plane_vox * 4, out16);
-          } else if constexpr (TAIL) {
-            head_blend_16(v, p.tail, s_head, pp, z, y0 + r, x0 + col);
-          } else {
-            store16(v, cb, ((size_t)z * p.Y + (y0 + r)) * p.X + (x0 + col), plane_vox, out16);
+        if constexpr (FMT != kFmtF16) {
+          if constexpr (FMT == kFmtF16x2) {  // same registers, different shape: let the first group complete
+            wg_commit();
+            wg_wait<0>();
+#pragma unroll
+            for (int g = 0; g < NTL; ++g) acc_fence(acc[g]);
+            wg_fence();
           }
-        }
-        if constexpr (MODE == kConvPool) {  // (1,2,2) max pool of the same values (y0, x0, TY, XT and the extents are even)
-          const int PX = p.XT / 2, npool = (p.TY / 2) * PX;
-          for (int item = tid; item < npool * (COUT / 16); item += nthr) {
-            const int pi = item % npool, cb = item / npool;
-            const int pr = pi / PX, pc = pi - pr * PX;
-            if (2 * pr >= ty_valid || 2 * pc >= xt_valid) continue;
-            float m[16], v[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) m[i] = -INFINITY;
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              load16((2 * pr + (k >> 1)) * p.pitch + 2 * pc + (k & 1), cb, v);
-#pragma unroll
-              for (int i = 0; i < 16; ++i) m[i] = fmaxf(m[i], v[i]);
-            }
-            const size_t pvox = ((size_t)z * (p.Y / 2) + (y0 / 2 + pr)) * (p.X / 2) + (x0 / 2 + pc);
-            store16(m, cb, pvox, plane_vox / 4, reinterpret_cast<uint4*>(p.out_pool));
-          }
-        }
-        if (MODE == kConvPool) named_sync(3, 256); else named_sync(1 + cw, 128);
-      }
-    };
-    if (MODE == kConvT && zz == 0) mbar_wait(BAR(kAF + 0), 0);  // plane z0 - 1 (unused) must have landed before its slot is freed
-    // conv: 27 taps accumulate into one job; convT: the 4 output parities are 4 jobs on the centre tap of plane z
-    for (int t = 0; t < NT; ++t) {
-      const int dz = MODE == kConvT ? 1 : t / 9, dy = MODE == kConvT ? 1 : (t / 3) % 3, dx = MODE == kConvT ? 1 : t % 3;
-      const int q = zz + dz, slot = q % kRing;
-      if (MODE == kConvT ? t == 0 : (dy == 0 && dx == 0)) mbar_wait(BAR(kAF + slot), (uint32_t)(q / kRing) & 1u);
-      const uint32_t a_slot = sA0 + (uint32_t)slot * p.slot_stride;
-      if (MODE == kConvT && t > 0) {
-#pragma unroll
-        for (int g = 0; g < MT; ++g)
-#pragma unroll
-          for (int i = 0; i < NA / 2; ++i) acc[g][i] = 0.f;
-      }
-      {
-        {
-          const int tap = t;
-          uint32_t st;
-          if (resident) {
-            st = (uint32_t)tap;
-            if (zz == 0) mbar_wait(BAR(kBF + st), 0);  // taps arrive once
-          } else {
-            st = ring_st;
-            mbar_wait(BAR(kBF + st), ring_parity);
-            if (++ring_st == nbs) { ring_st = 0; ring_parity ^= 1; }
-          }
-          const uint32_t b_tap = sB0 + st * Cfg::TAP;
-          const uint32_t a_tap = a_slot + (uint32_t)(dy * pitch + dx) * 16u;
-#pragma unroll
-          for (int g = 0; g < MT; ++g) acc_fence(acc[g]);
-          wg_fence();
-          // main products; accumulator accesses are ordered only between wgmma of the same shape, so the f16x2 second
-          // products (same registers, different shape) wait for the first group; the f16f8 e4m3 products use their own half
 #pragma unroll
           for (int ks = 0; ks < Cfg::KS; ++ks) {
             const uint32_t b_blk = b_tap + (uint32_t)ks * Cfg::BLK;
-            const uint32_t a_ks = a_tap + (uint32_t)(2 * ks * P) * p.plane_stride;
+            const uint32_t a_ks = a_tap + (uint32_t)(2 * ks * P + 1) * p.plane_stride;  // part 1: a_lo / [A8 | L8]
 #pragma unroll
-            for (int g = 0; g < MT; ++g) {
-              if (g < ntiles) {
-                const uint32_t a = a_ks + (uint32_t)((g0 + g) * 64) * 16u;
-                if constexpr (FMT == kFmtF16x2) wgmma_f16<2 * COUT>(acc[g], gdesc(a, a_lbo), gdesc(b_blk, 2 * COUT * 16), 1);
-                else wgmma_f16<COUT>(reinterpret_cast<float(&)[COUT / 2]>(acc[g]), gdesc(a, a_lbo), gdesc(b_blk, COUT * 16), 1);
-              }
+            for (int g = 0; g < NTL; ++g) {
+              const uint32_t a = a_ks + (uint32_t)((g0 + g) * 64) * 16u;
+              if constexpr (FMT == kFmtF16x2)
+                wgmma_f16<COUT>(reinterpret_cast<float(&)[COUT / 2]>(acc[g]), gdesc(a, a_lbo), gdesc(b_blk, 2 * COUT * 16), 1);
+              else
+                wgmma_e4m3<COUT>(reinterpret_cast<float(&)[COUT / 2]>(acc[g][COUT / 2]), gdesc(a, a_lbo),
+                                 gdesc(b_blk + 32 * COUT, COUT * 16), ks == 0 && first ? 0 : 1);
             }
-          }
-          if constexpr (FMT != kFmtF16) {
-            if constexpr (FMT == kFmtF16x2) {  // same registers, different shape: let the first group complete
-              wg_commit();
-              wg_wait<0>();
-            }
-#pragma unroll
-            for (int g = 0; g < MT; ++g) acc_fence(acc[g]);
-            wg_fence();
-#pragma unroll
-            for (int ks = 0; ks < Cfg::KS; ++ks) {
-              const uint32_t b_blk = b_tap + (uint32_t)ks * Cfg::BLK;
-              const uint32_t a_ks = a_tap + (uint32_t)(2 * ks * P + 1) * p.plane_stride;  // part 1: a_lo / [A8 | L8]
-#pragma unroll
-              for (int g = 0; g < MT; ++g) {
-                if (g < ntiles) {
-                  const uint32_t a = a_ks + (uint32_t)((g0 + g) * 64) * 16u;
-                  if constexpr (FMT == kFmtF16x2)
-                    wgmma_f16<COUT>(reinterpret_cast<float(&)[COUT / 2]>(acc[g]), gdesc(a, a_lbo), gdesc(b_blk, 2 * COUT * 16), 1);
-                  else
-                    wgmma_e4m3<COUT>(reinterpret_cast<float(&)[COUT / 2]>(acc[g][COUT / 2]), gdesc(a, a_lbo),
-                                     gdesc(b_blk + 32 * COUT, COUT * 16));
-                }
-              }
-            }
-          }
-          wg_commit();
-#pragma unroll
-          for (int g = 0; g < MT; ++g) acc_fence(acc[g]);
-          if (!resident) {
-            wg_wait<1>();  // the previous tap's products are done: its stage may be refilled
-            if (prev_st >= 0 && leader) mbar_arrive(BAR(kBE + prev_st));
-            prev_st = (int)st;
           }
         }
+        wg_commit();
+        // one tap of products stays in flight: the previous tap's are done, so its weight stage may be refilled and, once the
+        // last dz = 0 tap (t = 8) is done, the ring slot of plane z - 1
+        wg_wait<1>();
+#pragma unroll
+        for (int g = 0; g < NTL; ++g) acc_fence(acc[g]);
+        if (!resident) {
+          if (prev_st >= 0 && leader) mbar_arrive(BAR(kBE + prev_st));
+          prev_st = (int)st;
+        }
+        if (MODE != kConvT && t == 9 && leader) mbar_arrive(BAR(kAE + (zz % kRing)));
+        if (MODE == kConvT) epilogue(t);
       }
-      if (MODE == kConvT) epilogue(t);
+      if (MODE != kConvT) epilogue(0);
+      if (MODE == kConvT && leader) mbar_arrive(BAR(kAE + (zz % kRing)));  // plane z-1 (unused) is done with
     }
-    if (MODE != kConvT) epilogue(0);
-    if (MODE == kConvT && leader) mbar_arrive(BAR(kAE + (zz % kRing)));  // plane z-1 (unused) is done with
-  }
+  });
 }
 
 // ------------------------------------------------------------------------------------------

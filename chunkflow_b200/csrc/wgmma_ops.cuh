@@ -8,9 +8,9 @@ namespace cfb {
 // D (+)= A * B, fp16 operands from shared memory (K = 16); acc = 0 overwrites D
 template <int N>
 __device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t a, uint64_t b, int acc);
-// D += A * B, e4m3 operands from shared memory (K = 32)
+// D (+)= A * B, e4m3 operands from shared memory (K = 32); acc = 0 overwrites D
 template <int N>
-__device__ __forceinline__ void wgmma_e4m3(float (&d)[N / 2], uint64_t a, uint64_t b);
+__device__ __forceinline__ void wgmma_e4m3(float (&d)[N / 2], uint64_t a, uint64_t b, int acc);
 
 template <>
 __device__ __forceinline__ void wgmma_f16<16>(float (&d)[16 / 2], uint64_t a, uint64_t b, int acc) {
@@ -45,27 +45,27 @@ __device__ __forceinline__ void wgmma_f16<128>(float (&d)[128 / 2], uint64_t a, 
       : "l"(a), "l"(b), "r"(acc));
 }
 template <>
-__device__ __forceinline__ void wgmma_e4m3<16>(float (&d)[16 / 2], uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma_e4m3<16>(float (&d)[16 / 2], uint64_t a, uint64_t b, int acc) {
   asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
       "wgmma.mma_async.sync.aligned.m64n16k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-      : "l"(a), "l"(b));
+      : "l"(a), "l"(b), "r"(acc));
 }
 template <>
-__device__ __forceinline__ void wgmma_e4m3<32>(float (&d)[32 / 2], uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma_e4m3<32>(float (&d)[32 / 2], uint64_t a, uint64_t b, int acc) {
   asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
       "wgmma.mma_async.sync.aligned.m64n32k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(a), "l"(b));
+      : "l"(a), "l"(b), "r"(acc));
 }
 template <>
-__device__ __forceinline__ void wgmma_e4m3<64>(float (&d)[64 / 2], uint64_t a, uint64_t b) {
+__device__ __forceinline__ void wgmma_e4m3<64>(float (&d)[64 / 2], uint64_t a, uint64_t b, int acc) {
   asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
       "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n}\n"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(a), "l"(b));
+      : "l"(a), "l"(b), "r"(acc));
 }
 }  // namespace cfb
