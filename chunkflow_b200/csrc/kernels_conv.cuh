@@ -48,11 +48,12 @@ void free_packed(PackedConv& p);
 // and srcB (cb channels, may be null); all tensors CP8 in the layer's format.
 // If `tail` is given (16 -> 16 layers only) the epilogue does not store the activation but applies the
 // fused network tail: 1x1x1 head + sigmoid + crop + bump mask + red.global.add into the output chunk.
+// The blend steps of the other routes (network.cu) take their parameters from the same struct.
 struct ConvTail {
-  const float* head_w;      // device, (>= channels, 16)
+  const float* head_w;      // device, (>= channels, 16): the first `channels` rows are evaluated
   const float* head_b;      // device
   const PatchPos* patches;  // device, this batch
-  const float* mask;        // device, output patch mask
+  const float* mask;        // device, output patch mask (out_patch)
   float* out;               // device, (channels, out_size)
   int channels;
   Int3 out_patch, crop, out_size;
@@ -76,14 +77,12 @@ struct FirstConvW {
 };
 
 // First layer: extract `nb` patches from the uint8/f32 chunk (normalised by 1/255), 3x3x3
-// convolution 1 -> 16 in fp32 on CUDA cores, ReLU, CP8 output.  w: (16,1,3,3,3) fp32.
-// `cw` (host copy of the same weights) selects the constant-operand kernel; nullptr = weights staged in shared memory.
+// convolution 1 -> 16 in fp32 on CUDA cores, ReLU, CP8 output.
 void launch_first_conv_cp8(const void* chunk, int in_dtype, Int3 chunk_size, const PatchPos* patches, int nb,
-                           Int3 patch, const float* w, const float* bias, __half* out, int parts, cudaStream_t s,
-                           const FirstConvW* cw = nullptr);
+                           Int3 patch, const FirstConvW& w, __half* out, int parts, cudaStream_t s);
 // Same from already extracted fp32 patches (nb,1,Z,Y,X) (plugin level / debug).
-void launch_first_conv_cp8_from_patches(const float* patches, int nb, Int3 patch, const float* w, const float* bias,
-                                        __half* out, int parts, cudaStream_t s);
+void launch_first_conv_cp8_from_patches(const float* patches, int nb, Int3 patch, const FirstConvW& w, __half* out,
+                                        int parts, cudaStream_t s);
 
 void launch_maxpool_cp8(const __half* in, __half* out, int channels, int parts, int nb, Int3 in_size, cudaStream_t s);
 // ConvTranspose kernel=stride=(1,2,2), fp32 math on CUDA cores.  w: (cin, cout, 1,2,2) fp32.

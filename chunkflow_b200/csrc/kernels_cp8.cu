@@ -107,16 +107,14 @@ cp8_to_planar_kernel(const uint4* __restrict__ in, float* __restrict__ out, int 
 }
 
 // ---- first layer: extract + normalise + conv 1->16 + ReLU ---------------------------------
-// SRC: 0 = uint8 chunk, 1 = float chunk, 2 = float patches (nb,1,Z,Y,X)
+// SRC: 0 = uint8 chunk, 1 = float chunk, 2 = float patches (nb,1,Z,Y,X).  The weights are a kernel parameter (FirstConvW,
+// 1.8 KB in the constant bank), so every FFMA takes its weight as a constant-bank operand.
 constexpr int kFX = 32, kFY = 8;
 template <int SRC>
 __global__ void __launch_bounds__(kT)
 first_conv_cp8_kernel(const void* __restrict__ src, Int3 cs, const PatchPos* __restrict__ patches, Int3 ps,
-                      const float* __restrict__ w, const float* __restrict__ bias, uint4* __restrict__ out, int parts,
-                      int tiles_x) {
+                      const __grid_constant__ FirstConvW W, uint4* __restrict__ out, int parts, int tiles_x) {
   __shared__ float s_in[3][kFY + 2][kFX + 2];
-  __shared__ __align__(16) float s_w[27][16];
-  __shared__ float s_b[16];
   const int tile_x = blockIdx.x % tiles_x, tile_y = blockIdx.x / tiles_x;
   const int z = blockIdx.y, b = blockIdx.z;
   const int x0 = tile_x * kFX, y0 = tile_y * kFY;
@@ -127,71 +125,14 @@ first_conv_cp8_kernel(const void* __restrict__ src, Int3 cs, const PatchPos* __r
     const int gz = z + d - 1, gy = y0 + r - 1, gx = x0 + c - 1;
     float v = 0.f;  // zero padding at the PATCH border
     if (gz >= 0 && gz < ps.z && gy >= 0 && gy < ps.y && gx >= 0 && gx < ps.x) {
-      int sy = gy, sx = gx;
-      if (SRC != 2 && flags) tta_map(flags, ps.y, ps.x, gy, gx, sy, sx);  // augmented variant reads the original patch
-      if (SRC == 0) {
-        v = __fdiv_rn((float)static_cast<const uint8_t*>(src)[((size_t)(oz + gz) * cs.y + (oy + sy)) * cs.x + ox + sx], 255.0f);
-      } else if (SRC == 1) {
-        v = static_cast<const float*>(src)[((size_t)(oz + gz) * cs.y + (oy + sy)) * cs.x + ox + sx];
-      } else {
+      if (SRC == 2) {
         v = static_cast<const float*>(src)[(((size_t)b * ps.z + gz) * ps.y + gy) * ps.x + gx];
+      } else {
+        int sy = gy, sx = gx;
+        if (flags) tta_map(flags, ps.y, ps.x, gy, gx, sy, sx);  // augmented variant reads the original patch
+        const size_t idx = ((size_t)(oz + gz) * cs.y + (oy + sy)) * cs.x + ox + sx;
+        v = SRC == 0 ? __fdiv_rn((float)static_cast<const uint8_t*>(src)[idx], 255.0f) : static_cast<const float*>(src)[idx];
       }
-    }
-    s_in[d][r][c] = v;
-  }
-  for (int i = threadIdx.x; i < 27 * 16; i += kT) s_w[i / 16][i % 16] = w[(i % 16) * 27 + (i / 16)];
-  if (threadIdx.x < 16) s_b[threadIdx.x] = bias[threadIdx.x];
-  __syncthreads();
-  const int lx = threadIdx.x % kFX, ly = threadIdx.x / kFX;
-  const int x = x0 + lx, y = y0 + ly;
-  if (x >= ps.x || y >= ps.y) return;
-  float acc[16];
-#pragma unroll
-  for (int c = 0; c < 16; ++c) acc[c] = 0.f;
-#pragma unroll
-  for (int t = 0; t < 27; ++t) {
-    const float v = s_in[t / 9][ly + (t / 3) % 3][lx + t % 3];
-    const float4* wp = reinterpret_cast<const float4*>(&s_w[t][0]);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float4 wv = wp[q];
-      acc[q * 4 + 0] = fmaf(wv.x, v, acc[q * 4 + 0]);
-      acc[q * 4 + 1] = fmaf(wv.y, v, acc[q * 4 + 1]);
-      acc[q * 4 + 2] = fmaf(wv.z, v, acc[q * 4 + 2]);
-      acc[q * 4 + 3] = fmaf(wv.w, v, acc[q * 4 + 3]);
-    }
-  }
-  const size_t pvol = (size_t)ps.z * ps.y * ps.x;
-  const size_t vox = ((size_t)z * ps.y + y) * ps.x + x;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    float v[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { const float t = acc[h * 8 + i] + s_b[h * 8 + i]; v[i] = t < 0.f ? 0.f : t; }  // NaN passes, like torch.relu
-    store8(out, ((size_t)b * 2 + h) * fmt_planes(parts), parts, pvol, vox, v);
-  }
-}
-
-// Same layer with the weights as constant-bank operands (FirstConvW kernel parameter): identical FMA order and results.
-template <int SRC>
-__global__ void __launch_bounds__(kT)
-first_conv_cp8_const_kernel(const void* __restrict__ src, Int3 cs, const PatchPos* __restrict__ patches, Int3 ps,
-                            const __grid_constant__ FirstConvW W, uint4* __restrict__ out, int parts, int tiles_x) {
-  __shared__ float s_in[3][kFY + 2][kFX + 2];
-  const int tile_x = blockIdx.x % tiles_x, tile_y = blockIdx.x / tiles_x;
-  const int z = blockIdx.y, b = blockIdx.z;
-  const int x0 = tile_x * kFX, y0 = tile_y * kFY;
-  const PatchPos pp = patches[b];
-  const int oz = pp.iz, oy = pp.iy, ox = pp.ix, flags = pp.flags;
-  for (int i = threadIdx.x; i < 3 * (kFY + 2) * (kFX + 2); i += kT) {
-    const int c = i % (kFX + 2), r = (i / (kFX + 2)) % (kFY + 2), d = i / ((kFX + 2) * (kFY + 2));
-    const int gz = z + d - 1, gy = y0 + r - 1, gx = x0 + c - 1;
-    float v = 0.f;  // zero padding at the PATCH border
-    if (gz >= 0 && gz < ps.z && gy >= 0 && gy < ps.y && gx >= 0 && gx < ps.x) {
-      int sy = gy, sx = gx;
-      if (flags) tta_map(flags, ps.y, ps.x, gy, gx, sy, sx);  // augmented variant reads the original patch
-      const size_t idx = ((size_t)(oz + gz) * cs.y + (oy + sy)) * cs.x + ox + sx;
-      v = SRC == 0 ? __fdiv_rn((float)static_cast<const uint8_t*>(src)[idx], 255.0f) : static_cast<const float*>(src)[idx];
     }
     s_in[d][r][c] = v;
   }
@@ -379,30 +320,22 @@ void launch_cp8_to_planar(const __half* in, float* out, int channels, int parts,
 }
 
 void launch_first_conv_cp8(const void* chunk, int in_dtype, Int3 cs, const PatchPos* patches, int nb, Int3 ps,
-                           const float* w, const float* bias, __half* out, int parts, cudaStream_t s, const FirstConvW* cw) {
+                           const FirstConvW& w, __half* out, int parts, cudaStream_t s) {
   const int tiles_x = ceil_div(ps.x, kFX), tiles_y = ceil_div(ps.y, kFY);
   dim3 grid(tiles_x * tiles_y, ps.z, nb);
-  if (cw) {
-    if (in_dtype == CFB_DTYPE_U8)
-      first_conv_cp8_const_kernel<0><<<grid, kT, 0, s>>>(chunk, cs, patches, ps, *cw, reinterpret_cast<uint4*>(out), parts, tiles_x);
-    else
-      first_conv_cp8_const_kernel<1><<<grid, kT, 0, s>>>(chunk, cs, patches, ps, *cw, reinterpret_cast<uint4*>(out), parts, tiles_x);
-    CFB_LAUNCH_CHECK();
-    return;
-  }
   if (in_dtype == CFB_DTYPE_U8)
-    first_conv_cp8_kernel<0><<<grid, kT, 0, s>>>(chunk, cs, patches, ps, w, bias, reinterpret_cast<uint4*>(out), parts, tiles_x);
+    first_conv_cp8_kernel<0><<<grid, kT, 0, s>>>(chunk, cs, patches, ps, w, reinterpret_cast<uint4*>(out), parts, tiles_x);
   else
-    first_conv_cp8_kernel<1><<<grid, kT, 0, s>>>(chunk, cs, patches, ps, w, bias, reinterpret_cast<uint4*>(out), parts, tiles_x);
+    first_conv_cp8_kernel<1><<<grid, kT, 0, s>>>(chunk, cs, patches, ps, w, reinterpret_cast<uint4*>(out), parts, tiles_x);
   CFB_LAUNCH_CHECK();
 }
 
-void launch_first_conv_cp8_from_patches(const float* patches, int nb, Int3 ps, const float* w, const float* bias,
-                                        __half* out, int parts, cudaStream_t s) {
+void launch_first_conv_cp8_from_patches(const float* patches, int nb, Int3 ps, const FirstConvW& w, __half* out, int parts,
+                                        cudaStream_t s) {
   const int tiles_x = ceil_div(ps.x, kFX), tiles_y = ceil_div(ps.y, kFY);
   dim3 grid(tiles_x * tiles_y, ps.z, nb);
-  first_conv_cp8_kernel<2><<<grid, kT, 0, s>>>(patches, Int3{0, 0, 0}, nullptr, ps, w, bias, reinterpret_cast<uint4*>(out),
-                                               parts, tiles_x);
+  first_conv_cp8_kernel<2><<<grid, kT, 0, s>>>(patches, Int3{0, 0, 0}, nullptr, ps, w, reinterpret_cast<uint4*>(out), parts,
+                                               tiles_x);
   CFB_LAUNCH_CHECK();
 }
 

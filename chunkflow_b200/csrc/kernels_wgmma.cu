@@ -130,19 +130,6 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// Fused network tail for the last 3x3x3 layer (Cout = 16): 1x1x1 head + sigmoid + crop + bump mask +
-// red.global.add into the output chunk, straight from the fp32 accumulator values.
-struct FusedTail {
-  const float* head_w;   // (channels, 16) first rows of the head weight
-  const float* head_b;   // (channels)
-  const PatchPos* patches;
-  const float* mask;     // (op.z, op.y, op.x)
-  float* out;            // (channels, os.z, os.y, os.x)
-  int channels;
-  Int3 op, crop, os;
-  float scale;
-};
-
 template <int COUT, bool SPLIT>
 __device__ __forceinline__ void store_cp8_16(const float (&v)[16], int cb, int b, size_t vox, size_t plane_vox,
                                              uint4* __restrict__ out16) {
@@ -179,17 +166,17 @@ __device__ __forceinline__ void store_cp8_16_f8(const float (&v)[16], int cb, in
   out16[(plane + 3) * plane_vox + vox] = l8;
 }
 
-__device__ __forceinline__ void head_blend_16(const float (&v)[16], const FusedTail& t, const float* __restrict__ s_head,
+__device__ __forceinline__ void head_blend_16(const float (&v)[16], const ConvTail& t, const float* __restrict__ s_head,
                                               const PatchPos& pp, int z, int y, int x) {
   const int oz = z - t.crop.z, oy = y - t.crop.y, ox = x - t.crop.x;  // coordinates in the cropped output patch
-  if (oz < 0 || oz >= t.op.z || oy < 0 || oy >= t.op.y || ox < 0 || ox >= t.op.x) return;
+  if (oz < 0 || oz >= t.out_patch.z || oy < 0 || oy >= t.out_patch.y || ox < 0 || ox >= t.out_patch.x) return;
   int sy = oy, sx = ox;
-  if (pp.flags) tta_map(pp.flags, t.op.y, t.op.x, oy, ox, sy, sx);  // augmented variant: write back un-transformed
+  if (pp.flags) tta_map(pp.flags, t.out_patch.y, t.out_patch.x, oy, ox, sy, sx);  // augmented variant: write back un-transformed
   const int gz = pp.oz + oz, gy = pp.oy + sy, gx = pp.ox + sx;
-  if (gz < 0 || gz >= t.os.z || gy < 0 || gy >= t.os.y || gx < 0 || gx >= t.os.x) return;  // clipped by the chunk
-  const float m = __ldg(t.mask + ((size_t)oz * t.op.y + oy) * t.op.x + ox) * t.scale;
-  float* dst = t.out + ((size_t)gz * t.os.y + gy) * t.os.x + gx;
-  const size_t out_vol = (size_t)t.os.z * t.os.y * t.os.x;
+  if (gz < 0 || gz >= t.out_size.z || gy < 0 || gy >= t.out_size.y || gx < 0 || gx >= t.out_size.x) return;  // clipped by the chunk
+  const float m = __ldg(t.mask + ((size_t)oz * t.out_patch.y + oy) * t.out_patch.x + ox) * t.scale;
+  float* dst = t.out + ((size_t)gz * t.out_size.y + gy) * t.out_size.x + gx;
+  const size_t out_vol = (size_t)t.out_size.z * t.out_size.y * t.out_size.x;
   if (t.channels == 3) {
     // the affinity head: three independent FMA chains; sigmoid with ex2.approx / rcp.approx (~1e-7 of the exact value,
     // the tolerance of this path is 1e-3)
@@ -249,7 +236,7 @@ struct WgConvParams {
   int bresident;    // 1: all 27 taps stay resident (loaded once per CTA), 0: streamed through a ring
   int zblk, zblocks; // output planes per CTA and blocks per column (a CTA walks z in [zblk * block, + zblk))
   __half* out_pool; // kConvPool: (1,2,2) max-pooled copy of the output (CP8 of Z x Y/2 x X/2)
-  FusedTail tail;   // used by the TAIL = true instantiations only
+  ConvTail tail;    // used by the TAIL = true instantiations only
 };
 
 // What a kernel instantiation computes: a 3x3x3 convolution, the same with the (1,2,2) max pool of its output fused into
@@ -681,7 +668,7 @@ ConvTile choose_tile(int nb, Int3 sz) {
 
 template <int CIN, int COUT, int FMT, int MODE>
 void launch_cfg(const __half* srcA, int ca, const __half* srcB, int cb, const PackedConv& w, __half* out, int nb,
-                Int3 sz, bool relu, cudaStream_t s, const FusedTail* tail, __half* pool_out = nullptr) {
+                Int3 sz, bool relu, cudaStream_t s, const ConvTail* tail, __half* pool_out = nullptr) {
   using Cfg = ConvCfg<CIN, COUT, FMT>;
   const uint64_t key = ((uint64_t)sz.z << 48) ^ ((uint64_t)sz.y << 32) ^ ((uint64_t)sz.x << 16) ^ (uint64_t)nb;
   auto it = w.tuned->find(key);
@@ -724,7 +711,7 @@ void launch_cfg(const __half* srcA, int ca, const __half* srcB, int cb, const Pa
 
 template <int FMT>
 void dispatch(const __half* srcA, int ca, const __half* srcB, int cb, const PackedConv& w, __half* out, int nb, Int3 sz,
-              bool relu, cudaStream_t s, const FusedTail* tail, __half* pool_out) {
+              bool relu, cudaStream_t s, const ConvTail* tail, __half* pool_out) {
   const int cin = ca + cb, cout = w.cout;
 #define CFB_CASE(CI, CO) \
   if (cin == CI && cout == CO) return launch_cfg<CI, CO, FMT, kConv>(srcA, ca, srcB, cb, w, out, nb, sz, relu, s, tail);
@@ -744,16 +731,10 @@ void launch_conv3_wgmma(const __half* srcA, int ca, const __half* srcB, int cb, 
                         Int3 sz, bool relu, cudaStream_t s, const ConvTail* tail, __half* pool_out) {
   if (ca % 16 || (cb % 16) || w.cin != ca + cb || w.taps != 27) throw std::runtime_error("conv3_wgmma: channel mismatch");
   if (pool_out && (tail || (sz.y & 1) || (sz.x & 1))) throw std::runtime_error("conv3_wgmma: pooling needs even y, x and no fused tail");
-  FusedTail ft{};
-  if (tail) {
-    if (tail->channels > 8) throw std::runtime_error("fused tail: at most 8 channels");
-    ft.head_w = tail->head_w; ft.head_b = tail->head_b; ft.patches = tail->patches; ft.mask = tail->mask; ft.out = tail->out;
-    ft.channels = tail->channels; ft.op = tail->out_patch; ft.crop = tail->crop; ft.os = tail->out_size;
-    ft.scale = tail->scale;
-  }
-  if (w.fmt == kFmtF16F8) dispatch<kFmtF16F8>(srcA, ca, srcB, cb, w, out, nb, sz, relu, s, tail ? &ft : nullptr, pool_out);
-  else if (w.fmt == kFmtF16x2) dispatch<kFmtF16x2>(srcA, ca, srcB, cb, w, out, nb, sz, relu, s, tail ? &ft : nullptr, pool_out);
-  else dispatch<kFmtF16>(srcA, ca, srcB, cb, w, out, nb, sz, relu, s, tail ? &ft : nullptr, pool_out);
+  if (tail && tail->channels > 8) throw std::runtime_error("fused tail: at most 8 channels");
+  if (w.fmt == kFmtF16F8) dispatch<kFmtF16F8>(srcA, ca, srcB, cb, w, out, nb, sz, relu, s, tail, pool_out);
+  else if (w.fmt == kFmtF16x2) dispatch<kFmtF16x2>(srcA, ca, srcB, cb, w, out, nb, sz, relu, s, tail, pool_out);
+  else dispatch<kFmtF16>(srcA, ca, srcB, cb, w, out, nb, sz, relu, s, tail, pool_out);
 }
 
 void launch_convT_wgmma(const __half* in, const PackedConv& w, __half* out, int nb, Int3 in_size, cudaStream_t s) {

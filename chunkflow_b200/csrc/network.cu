@@ -10,17 +10,41 @@
 namespace cfb {
 
 namespace {
-struct Spec {
-  const char* name;
-  int cin, cout, taps;  // taps: 27 conv3, 4 convT, 1 head
+enum Op { kOpFirst, kOpConv3, kOpConv3Pool, kOpConvT, kOpHead };
+struct Step {
+  const char* name;  // profiling name; "<name>.weight" and "<name>.bias" in the state dict
+  Op op;             // kOpFirst: 3x3x3 conv from the input patches; kOpConv3Pool: 3x3x3 conv feeding a (1,2,2) max pool
+  int cin, cout;     // cout -1: the head, whose channels come from its weight tensor
+  Act a, b;          // source, and the skip connection concatenated after it (torch.cat([a, b]))
+  Act dst, pool;     // output, and its (1,2,2) max pool
+  int level;         // resolution of the sources: the patch, then (Y/2, X/2) and (Y/4, X/4)
 };
-// execution order; cout -1 = head (num channels from the weight tensor)
-const Spec kSpecs[] = {
-    {"enc0.0", 1, 16, 27},  {"enc0.2", 16, 16, 27}, {"enc1.0", 16, 32, 27}, {"enc1.2", 32, 32, 27},
-    {"enc2.0", 32, 64, 27}, {"enc2.2", 64, 64, 27}, {"up1", 64, 32, 4},     {"dec1.0", 64, 32, 27},
-    {"dec1.2", 32, 32, 27}, {"up0", 32, 16, 4},     {"dec0.0", 32, 16, 27}, {"dec0.2", 16, 16, 27},
-    {"head", 16, -1, 1},
+// execution order
+const Step kNet[] = {
+    {"enc0.0", kOpFirst, 1, 16, kIn, kNoAct, kE0a, kNoAct, 0},
+    {"enc0.2", kOpConv3Pool, 16, 16, kE0a, kNoAct, kE0, kP0, 0},
+    {"enc1.0", kOpConv3, 16, 32, kP0, kNoAct, kE1a, kNoAct, 1},
+    {"enc1.2", kOpConv3Pool, 32, 32, kE1a, kNoAct, kE1, kP1, 1},
+    {"enc2.0", kOpConv3, 32, 64, kP1, kNoAct, kE2a, kNoAct, 2},
+    {"enc2.2", kOpConv3, 64, 64, kE2a, kNoAct, kE2, kNoAct, 2},
+    {"up1", kOpConvT, 64, 32, kE2, kNoAct, kU1, kNoAct, 2},
+    {"dec1.0", kOpConv3, 64, 32, kU1, kE1, kD1a, kNoAct, 1},
+    {"dec1.2", kOpConv3, 32, 32, kD1a, kNoAct, kD1, kNoAct, 1},
+    {"up0", kOpConvT, 32, 16, kD1, kNoAct, kU0, kNoAct, 1},
+    {"dec0.0", kOpConv3, 32, 16, kU0, kE0, kD0a, kNoAct, 0},
+    {"dec0.2", kOpConv3, 16, 16, kD0a, kNoAct, kD0, kNoAct, 0},
+    {"head", kOpHead, 16, -1, kD0, kNoAct, kOut, kNoAct, 0},
 };
+constexpr int kSteps = sizeof(kNet) / sizeof(kNet[0]);
+const char* const kPoolName[] = {"pool0", "pool1"};  // by level
+
+int taps(Op op) { return op == kOpConvT ? 4 : op == kOpHead ? 1 : 27; }
+// channels of an activation: the input patches have one, every other one those of the step that produces it
+int act_channels(Act a) {
+  for (const Step& st : kNet)
+    if (st.dst == a || st.pool == a) return st.cout;
+  return 1;
+}
 }  // namespace
 
 void Network::configure(int precision, Int3 patch, int batch) {
@@ -35,90 +59,71 @@ void Network::configure(int precision, Int3 patch, int batch) {
 void Network::release() {
   for (void* p : owned_) cudaFree(p);
   owned_.clear();
-  for (auto& kv : layers_) { cudaFree(kv.second.w); cudaFree(kv.second.bias); free_packed(kv.second.packed); }
+  for (ConvLayer& L : layers_) { cudaFree(L.w); cudaFree(L.bias); free_packed(L.packed); }
   layers_.clear();
   for (cudaEvent_t e : prof_pool_) cudaEventDestroy(e);
   prof_pool_.clear();
   ready_ = false;
-  buf_in_ = nullptr;
-  e0a_ = nullptr;
+  act_.fill(nullptr);
 }
 
 float* Network::patch_input_buffer(int nb) {
   if (nb > batch_) throw std::invalid_argument("batch larger than configured");
-  if (!buf_in_) {
-    CFB_CUDA(cudaMalloc(&buf_in_, (size_t)vol(patch_) * batch_ * sizeof(float)));
-    owned_.push_back(buf_in_);
+  if (!act_[kIn]) {
+    CFB_CUDA(cudaMalloc(&act_[kIn], (size_t)vol(patch_) * batch_ * sizeof(float)));
+    owned_.push_back(act_[kIn]);
   }
-  return buf_in_;
+  return f32(kIn);
 }
 
 void Network::allocate() {
-  if (e0a_) return;
-  const int64_t v0 = vol(patch_), v1 = v0 / 4, v2 = v0 / 16;
-  auto alloc = [&](int64_t floats) {
-    float* p = nullptr;
-    CFB_CUDA(cudaMalloc(&p, (size_t)floats * batch_ * sizeof(float)));
-    owned_.push_back(p);
-    return p;
-  };
+  if (act_[kOut]) return;
   patch_input_buffer(1);
-  net_out_ = alloc((int64_t)std::max(cnet_, 1) * v0);
-  if (umma()) {
-    const int P = parts();
-    auto halloc = [&](int64_t channels, int64_t v) {
-      __half* p = nullptr;
-      CFB_CUDA(cudaMalloc(&p, (size_t)channels * P * v * batch_ * sizeof(__half)));
-      owned_.push_back(p);
-      return p;
-    };
-    h_e0a_ = halloc(16, v0); h_e0_ = halloc(16, v0); h_p0_ = halloc(16, v1);
-    h_e1a_ = halloc(32, v1); h_e1_ = halloc(32, v1); h_p1_ = halloc(32, v2);
-    h_e2a_ = halloc(64, v2); h_e2_ = halloc(64, v2);
-    h_u1_ = halloc(32, v1); h_d1a_ = halloc(32, v1); h_d1_ = halloc(32, v1);
-    h_u0_ = halloc(16, v0); h_d0a_ = halloc(16, v0); h_d0_ = halloc(16, v0);
-    e0a_ = net_out_;  // marks "allocated"
-    return;
+  auto alloc = [&](Act a, size_t bytes_per_voxel, int level) {
+    CFB_CUDA(cudaMalloc(&act_[a], bytes_per_voxel * (size_t)(vol(patch_) >> (2 * level)) * batch_));
+    owned_.push_back(act_[a]);
+  };
+  alloc(kOut, sizeof(float) * std::max(cnet_, 1), 0);
+  const size_t bytes = tensor_cores() ? sizeof(__half) * parts() : sizeof(float);  // per channel and voxel
+  for (const Step& st : kNet) {
+    if (st.op == kOpHead) continue;
+    alloc(st.dst, bytes * st.cout, st.op == kOpConvT ? st.level - 1 : st.level);
+    if (st.pool != kNoAct) alloc(st.pool, bytes * st.cout, st.level + 1);
   }
-  e0a_ = alloc(16 * v0); e0_ = alloc(16 * v0); p0_ = alloc(16 * v1);
-  e1a_ = alloc(32 * v1); e1_ = alloc(32 * v1); p1_ = alloc(32 * v2);
-  e2a_ = alloc(64 * v2); e2_ = alloc(64 * v2);
-  u1_ = alloc(32 * v1); d1a_ = alloc(32 * v1); d1_ = alloc(32 * v1);
-  u0_ = alloc(16 * v0); d0a_ = alloc(16 * v0); d0_ = alloc(16 * v0);
 }
 
 bool Network::load(const std::map<std::string, std::vector<float>>& host_w, int num_output_channels, std::string& err) {
   ready_ = false;
-  for (auto& kv : layers_) { cudaFree(kv.second.w); cudaFree(kv.second.bias); free_packed(kv.second.packed); }
+  for (ConvLayer& L : layers_) { cudaFree(L.w); cudaFree(L.bias); free_packed(L.packed); }
   layers_.clear();
-  for (const Spec& sp : kSpecs) {
-    const std::string wn = std::string(sp.name) + ".weight", bn = std::string(sp.name) + ".bias";
+  for (const Step& st : kNet) {
+    const std::string wn = std::string(st.name) + ".weight", bn = std::string(st.name) + ".bias";
     auto wi = host_w.find(wn), bi = host_w.find(bn);
     if (wi == host_w.end() || bi == host_w.end()) { err = "missing tensor " + (wi == host_w.end() ? wn : bn); return false; }
-    int cout = sp.cout;
-    if (cout < 0) {
-      if (wi->second.size() % sp.cin) { err = "head.weight has a wrong size"; return false; }
-      cout = (int)(wi->second.size() / sp.cin);
+    const std::vector<float>& w = wi->second;
+    const std::vector<float>& b = bi->second;
+    int cout = st.cout;
+    if (st.op == kOpHead) {
+      if (w.size() % st.cin) { err = "head.weight has a wrong size"; return false; }
+      cout = (int)(w.size() / st.cin);
       cnet_ = cout;
     }
-    if ((int64_t)wi->second.size() != (int64_t)sp.cin * cout * sp.taps) { err = wn + " has a wrong size"; return false; }
-    if ((int)bi->second.size() != cout) { err = bn + " has a wrong size"; return false; }
+    if ((int64_t)w.size() != (int64_t)st.cin * cout * taps(st.op)) { err = wn + " has a wrong size"; return false; }
+    if ((int)b.size() != cout) { err = bn + " has a wrong size"; return false; }
     ConvLayer L;
-    L.name = sp.name; L.cin = sp.cin; L.cout = cout;
-    CFB_CUDA(cudaMalloc(&L.w, wi->second.size() * sizeof(float)));
-    CFB_CUDA(cudaMalloc(&L.bias, bi->second.size() * sizeof(float)));
-    CFB_CUDA(cudaMemcpy(L.w, wi->second.data(), wi->second.size() * sizeof(float), cudaMemcpyHostToDevice));
-    CFB_CUDA(cudaMemcpy(L.bias, bi->second.data(), bi->second.size() * sizeof(float), cudaMemcpyHostToDevice));
-    if (umma() && sp.taps == 27 && sp.cin >= 16)
-      pack_conv3_weights(wi->second.data(), bi->second.data(), sp.cin, cout, fmt(), L.packed);
-    if (umma() && sp.taps == 4)
-      pack_convT_weights(wi->second.data(), bi->second.data(), sp.cin, cout, fmt(), L.packed);
-    if (umma() && sp.taps == 27 && sp.cin == 1 && cout == 16) {
+    CFB_CUDA(cudaMalloc(&L.w, w.size() * sizeof(float)));
+    CFB_CUDA(cudaMalloc(&L.bias, b.size() * sizeof(float)));
+    CFB_CUDA(cudaMemcpy(L.w, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice));
+    CFB_CUDA(cudaMemcpy(L.bias, b.data(), b.size() * sizeof(float), cudaMemcpyHostToDevice));
+    if (tensor_cores() && (st.op == kOpConv3 || st.op == kOpConv3Pool))
+      pack_conv3_weights(w.data(), b.data(), st.cin, cout, fmt(), L.packed);
+    if (tensor_cores() && st.op == kOpConvT) pack_convT_weights(w.data(), b.data(), st.cin, cout, fmt(), L.packed);
+    if (tensor_cores() && st.op == kOpFirst) {
       for (int t = 0; t < 27; ++t)
-        for (int c = 0; c < 16; ++c) first_w_.w[t][c] = wi->second[(size_t)c * 27 + t];
-      for (int c = 0; c < 16; ++c) first_w_.b[c] = bi->second[c];
+        for (int c = 0; c < 16; ++c) first_w_.w[t][c] = w[(size_t)c * 27 + t];
+      for (int c = 0; c < 16; ++c) first_w_.b[c] = b[c];
     }
-    layers_[sp.name] = L;
+    layers_.push_back(L);
   }
   if (num_output_channels > cnet_) { err = "the network produces fewer channels than num_output_channels"; return false; }
   if (cnet_ > 8) { err = "at most 8 network output channels are supported"; return false; }
@@ -170,133 +175,96 @@ void Network::layer_timing(std::vector<std::string>& names, std::vector<float>& 
   names = prof_names_; ms = prof_ms_; launches = prof_launches_;
 }
 
-int Network::forward(int nb, cudaStream_t s) {
-  const Int3 s0 = patch_, s1{patch_.z, patch_.y / 2, patch_.x / 2}, s2{patch_.z, patch_.y / 4, patch_.x / 4};
-  auto conv = [&](const char* name, const float* a, int ca, const float* b, int cb, float* out, Int3 sz) {
-    const ConvLayer& L = layers_.at(name);
-    prof_begin(name, s);
-    launch_conv3_f32(a, ca, b, cb, L.w, L.bias, out, L.cout, nb, sz, /*relu=*/true, s);
-    prof_end(s);
-  };
-  conv("enc0.0", buf_in_, 1, nullptr, 0, e0a_, s0);
-  conv("enc0.2", e0a_, 16, nullptr, 0, e0_, s0);
-  prof_begin("pool0", s); launch_maxpool_f32(e0_, p0_, 16, nb, s0, s); prof_end(s);
-  conv("enc1.0", p0_, 16, nullptr, 0, e1a_, s1);
-  conv("enc1.2", e1a_, 32, nullptr, 0, e1_, s1);
-  prof_begin("pool1", s); launch_maxpool_f32(e1_, p1_, 32, nb, s1, s); prof_end(s);
-  conv("enc2.0", p1_, 32, nullptr, 0, e2a_, s2);
-  conv("enc2.2", e2a_, 64, nullptr, 0, e2_, s2);
-  { const ConvLayer& L = layers_.at("up1"); prof_begin("up1", s); launch_convT_f32(e2_, L.w, L.bias, u1_, 64, 32, nb, s2, s); prof_end(s); }
-  conv("dec1.0", u1_, 32, e1_, 32, d1a_, s1);  // torch.cat([up1, enc1])
-  conv("dec1.2", d1a_, 32, nullptr, 0, d1_, s1);
-  { const ConvLayer& L = layers_.at("up0"); prof_begin("up0", s); launch_convT_f32(d1_, L.w, L.bias, u0_, 32, 16, nb, s1, s); prof_end(s); }
-  conv("dec0.0", u0_, 16, e0_, 16, d0a_, s0);  // torch.cat([up0, enc0])
-  conv("dec0.2", d0a_, 16, nullptr, 0, d0_, s0);
-  { const ConvLayer& L = layers_.at("head"); prof_begin("head", s); launch_head_sigmoid_f32(d0_, L.w, L.bias, net_out_, 16, cnet_, nb, s0, s); prof_end(s); }
-  return 15;
+Network::CrossChecks Network::read_cross_checks() {
+  return {getenv("CFB_NO_POOL_FUSION") != nullptr, getenv("CFB_SIMT_CONVT") != nullptr, getenv("CFB_NO_FUSED_TAIL") != nullptr};
 }
 
-int Network::forward_cp8(const void* chunk, int in_dtype, Int3 cs, const PatchPos* patches, int nb, cudaStream_t s,
-                         bool with_head, const ConvTail* tail) {
-  const Int3 s0 = patch_, s1{patch_.z, patch_.y / 2, patch_.x / 2}, s2{patch_.z, patch_.y / 4, patch_.x / 4};
+int Network::run(const Route& r, int nb, cudaStream_t s) {
+  const bool tc = tensor_cores();
   const int P = fmt();  // the CUDA-core CP8 kernels take the number format
-  {
-    const ConvLayer& L = layers_.at("enc0.0");
-    prof_begin("enc0.0", s);
-    if (chunk) launch_first_conv_cp8(chunk, in_dtype, cs, patches, nb, s0, L.w, L.bias, h_e0a_, P, s,
-                                     getenv("CFB_FIRST_CONV_SMEM_W") ? nullptr : &first_w_);
-    else launch_first_conv_cp8_from_patches(buf_in_, nb, s0, L.w, L.bias, h_e0a_, P, s);
-    prof_end(s);
-  }
-  auto conv = [&](const char* name, const __half* a, int ca, const __half* b, int cb, __half* out, Int3 sz, __half* pool_out = nullptr) {
-    const ConvLayer& L = layers_.at(name);
+  ConvTail blend = r.blend;
+  blend.head_w = layers_[kSteps - 1].w;
+  blend.head_b = layers_[kSteps - 1].bias;
+  int launches = 0;
+  auto issue = [&](const char* name, auto&& launch) {
     prof_begin(name, s);
-    launch_conv3_wgmma(a, ca, b, cb, L.packed, out, nb, sz, /*relu=*/true, s, nullptr, pool_out);
+    launch();
     prof_end(s);
+    ++launches;
   };
-  // the two encoder outputs feed a (1,2,2) max pool: fused into the convolution's epilogue unless CFB_NO_POOL_FUSION is set
-  const bool fuse_pool = getenv("CFB_NO_POOL_FUSION") == nullptr;
-  int launches_saved = 0;
-  conv("enc0.2", h_e0a_, 16, nullptr, 0, h_e0_, s0, fuse_pool ? h_p0_ : nullptr);
-  if (!fuse_pool) { prof_begin("pool0", s); launch_maxpool_cp8(h_e0_, h_p0_, 16, P, nb, s0, s); prof_end(s); } else ++launches_saved;
-  conv("enc1.0", h_p0_, 16, nullptr, 0, h_e1a_, s1);
-  conv("enc1.2", h_e1a_, 32, nullptr, 0, h_e1_, s1, fuse_pool ? h_p1_ : nullptr);
-  if (!fuse_pool) { prof_begin("pool1", s); launch_maxpool_cp8(h_e1_, h_p1_, 32, P, nb, s1, s); prof_end(s); } else ++launches_saved;
-  conv("enc2.0", h_p1_, 32, nullptr, 0, h_e2a_, s2);
-  conv("enc2.2", h_e2a_, 64, nullptr, 0, h_e2_, s2);
-  // transposed convolutions on wgmma; CFB_SIMT_CONVT selects the CUDA-core kernel (fp32 math, a cross-check)
-  const bool simt_up = getenv("CFB_SIMT_CONVT") != nullptr;
-  { const ConvLayer& L = layers_.at("up1"); prof_begin("up1", s);
-    if (simt_up) launch_convT_cp8(h_e2_, L.w, L.bias, h_u1_, 64, 32, P, nb, s2, s); else launch_convT_wgmma(h_e2_, L.packed, h_u1_, nb, s2, s);
-    prof_end(s); }
-  conv("dec1.0", h_u1_, 32, h_e1_, 32, h_d1a_, s1);  // torch.cat([up1, enc1])
-  conv("dec1.2", h_d1a_, 32, nullptr, 0, h_d1_, s1);
-  { const ConvLayer& L = layers_.at("up0"); prof_begin("up0", s);
-    if (simt_up) launch_convT_cp8(h_d1_, L.w, L.bias, h_u0_, 32, 16, P, nb, s1, s); else launch_convT_wgmma(h_d1_, L.packed, h_u0_, nb, s1, s);
-    prof_end(s); }
-  conv("dec0.0", h_u0_, 16, h_e0_, 16, h_d0a_, s0);  // torch.cat([up0, enc0])
-  if (tail) {  // 3x3x3 conv + ReLU + 1x1x1 head + sigmoid + crop + bump mask + blend in one kernel
-    const ConvLayer& L = layers_.at("dec0.2");
-    prof_begin("dec0.2+head+blend", s);
-    launch_conv3_wgmma(h_d0a_, 16, nullptr, 0, L.packed, h_d0_, nb, s0, /*relu=*/true, s, tail);
-    prof_end(s);
-    return 14 - launches_saved;
+  for (int i = 0; i < kSteps; ++i) {
+    const Step& st = kNet[i];
+    const ConvLayer& L = layers_[i];
+    const Int3 sz{patch_.z, patch_.y >> st.level, patch_.x >> st.level};
+    const int cb = st.b == kNoAct ? 0 : act_channels(st.b), ca = st.cin - cb;
+    if (st.op == kOpFirst) {
+      if (!tc && r.chunk)
+        issue("extract", [&] { launch_extract_patches(r.chunk, r.in_dtype, r.chunk_size, blend.patches, nb, patch_, f32(kIn), s); });
+      issue(st.name, [&] {
+        if (!tc) launch_conv3_f32(f32(kIn), 1, nullptr, 0, L.w, L.bias, f32(st.dst), st.cout, nb, sz, /*relu=*/true, s);
+        else if (r.chunk) launch_first_conv_cp8(r.chunk, r.in_dtype, r.chunk_size, blend.patches, nb, sz, first_w_, cp8(st.dst), P, s);
+        else launch_first_conv_cp8_from_patches(f32(kIn), nb, sz, first_w_, cp8(st.dst), P, s);
+      });
+    } else if (st.op == kOpConv3 || st.op == kOpConv3Pool) {
+      const bool pool = st.op == kOpConv3Pool, fuse_pool = tc && pool && !r.checks.no_pool_fusion;
+      const bool fuse_tail = r.end == kFusedTail && kNet[i + 1].op == kOpHead;  // + head + sigmoid + crop + mask + blend
+      issue(fuse_tail ? (std::string(st.name) + "+head+blend").c_str() : st.name, [&] {
+        if (!tc) launch_conv3_f32(f32(st.a), ca, cb ? f32(st.b) : nullptr, cb, L.w, L.bias, f32(st.dst), st.cout, nb, sz, true, s);
+        else launch_conv3_wgmma(cp8(st.a), ca, cb ? cp8(st.b) : nullptr, cb, L.packed, cp8(st.dst), nb, sz, /*relu=*/true, s,
+                                fuse_tail ? &blend : nullptr, fuse_pool ? cp8(st.pool) : nullptr);
+      });
+      if (pool && !fuse_pool)
+        issue(kPoolName[st.level], [&] {
+          if (tc) launch_maxpool_cp8(cp8(st.dst), cp8(st.pool), st.cout, P, nb, sz, s);
+          else launch_maxpool_f32(f32(st.dst), f32(st.pool), st.cout, nb, sz, s);
+        });
+    } else if (st.op == kOpConvT) {
+      issue(st.name, [&] {
+        if (!tc) launch_convT_f32(f32(st.a), L.w, L.bias, f32(st.dst), st.cin, st.cout, nb, sz, s);
+        else if (r.checks.simt_convt) launch_convT_cp8(cp8(st.a), L.w, L.bias, cp8(st.dst), st.cin, st.cout, P, nb, sz, s);
+        else launch_convT_wgmma(cp8(st.a), L.packed, cp8(st.dst), nb, sz, s);
+      });
+    } else if (r.end == kBlend && tc) {
+      issue("head+blend", [&] {
+        launch_head_blend_cp8(cp8(st.a), L.w, L.bias, st.cin, cnet_, P, sz, blend.out_patch, blend.crop, blend.mask, blend.patches,
+                              nb, blend.out, blend.channels, blend.out_size, blend.scale, s);
+      });
+    } else if (r.end != kFusedTail) {
+      issue(st.name, [&] {
+        if (tc) launch_head_sigmoid_cp8(cp8(st.a), L.w, L.bias, f32(st.dst), st.cin, cnet_, P, nb, sz, s);
+        else launch_head_sigmoid_f32(f32(st.a), L.w, L.bias, f32(st.dst), st.cin, cnet_, nb, sz, s);
+      });
+      if (r.end == kBlend)
+        issue("blend", [&] {
+          launch_blend_patches(f32(st.dst), cnet_, patch_, blend.out_patch, blend.crop, blend.mask, blend.patches, nb, blend.out,
+                               blend.channels, blend.out_size, blend.scale, s);
+        });
+    }
   }
-  conv("dec0.2", h_d0a_, 16, nullptr, 0, h_d0_, s0);
-  if (!with_head) return 14 - launches_saved;  // the head is fused into the blend kernel
-  { const ConvLayer& L = layers_.at("head"); prof_begin("head", s); launch_head_sigmoid_cp8(h_d0_, L.w, L.bias, net_out_, 16, cnet_, P, nb, s0, s); prof_end(s); }
-  return 15 - launches_saved;
-}
-
-int Network::forward_from_chunk(const void* chunk, int in_dtype, Int3 cs, const PatchPos* patches, int nb, cudaStream_t s) {
-  if (nb > batch_) throw std::invalid_argument("batch larger than configured");
-  if (umma()) return forward_cp8(chunk, in_dtype, cs, patches, nb, s, /*with_head=*/false);
-  prof_begin("extract", s);
-  launch_extract_patches(chunk, in_dtype, cs, patches, nb, patch_, buf_in_, s);
-  prof_end(s);
-  return 1 + forward(nb, s);
+  return launches;
 }
 
 int Network::forward_and_blend(const void* chunk, int in_dtype, Int3 cs, const PatchPos* patches, int nb, Int3 op, Int3 crop,
                                const float* mask, float* out, int channels, Int3 out_size, float scale, cudaStream_t s) {
   if (nb > batch_) throw std::invalid_argument("batch larger than configured");
-  if (umma() && !getenv("CFB_NO_FUSED_TAIL")) {
-    const ConvLayer& H = layers_.at("head");
-    ConvTail tail{H.w, H.bias, patches, mask, out, channels, op, crop, out_size, scale};
-    return forward_cp8(chunk, in_dtype, cs, patches, nb, s, /*with_head=*/false, &tail);
-  }
-  int n = forward_from_chunk(chunk, in_dtype, cs, patches, nb, s);
-  return n + blend(op, crop, mask, patches, nb, out, channels, out_size, scale, s);
+  const CrossChecks checks = read_cross_checks();
+  const End end = tensor_cores() && !checks.no_fused_tail ? kFusedTail : kBlend;
+  return run(Route{chunk, in_dtype, cs, end, ConvTail{nullptr, nullptr, patches, mask, out, channels, op, crop, out_size, scale}, checks},
+             nb, s);
 }
 
 int Network::forward_from_host_patches(const float* h_patches, int nb, cudaStream_t s) {
   if (nb > batch_) throw std::invalid_argument("batch larger than configured");
-  CFB_CUDA(cudaMemcpyAsync(buf_in_, h_patches, (size_t)nb * vol(patch_) * sizeof(float), cudaMemcpyHostToDevice, s));
-  if (umma()) return forward_cp8(nullptr, 0, Int3{0, 0, 0}, nullptr, nb, s, /*with_head=*/true);
-  return forward(nb, s);
-}
-
-int Network::blend(Int3 op, Int3 crop, const float* mask, const PatchPos* patches, int nb, float* out, int channels,
-                   Int3 out_size, float scale, cudaStream_t s) {
-  if (umma()) {
-    const ConvLayer& L = layers_.at("head");
-    prof_begin("head+blend", s);
-    launch_head_blend_cp8(h_d0_, L.w, L.bias, 16, cnet_, fmt(), patch_, op, crop, mask, patches, nb, out, channels, out_size, scale, s);
-    prof_end(s);
-    return 1;
-  }
-  prof_begin("blend", s);
-  launch_blend_patches(net_out_, cnet_, patch_, op, crop, mask, patches, nb, out, channels, out_size, scale, s);
-  prof_end(s);
-  return 1;
+  CFB_CUDA(cudaMemcpyAsync(f32(kIn), h_patches, (size_t)nb * vol(patch_) * sizeof(float), cudaMemcpyHostToDevice, s));
+  return run(Route{nullptr, 0, Int3{0, 0, 0}, kRawOutput, ConvTail{}, read_cross_checks()}, nb, s);
 }
 
 void Network::crop_mask(Int3 op, Int3 crop, const float* mask, int nb, float* dst, int channels, cudaStream_t s) {
-  launch_crop_mask(net_out_, cnet_, patch_, op, crop, mask, nb, dst, channels, /*repeat=*/false, s);
+  launch_crop_mask(f32(kOut), cnet_, patch_, op, crop, mask, nb, dst, channels, /*repeat=*/false, s);
 }
 
 void Network::copy_raw_output_to_host(float* h_out, cudaStream_t s) {
-  CFB_CUDA(cudaMemcpyAsync(h_out, net_out_, (size_t)cnet_ * vol(patch_) * sizeof(float), cudaMemcpyDeviceToHost, s));
+  CFB_CUDA(cudaMemcpyAsync(h_out, f32(kOut), (size_t)cnet_ * vol(patch_) * sizeof(float), cudaMemcpyDeviceToHost, s));
 }
 
 int Network::debug_conv3(const float* h_in, int cin, Int3 size, const float* h_w, const float* h_b, int cout, bool relu,
@@ -310,7 +278,7 @@ int Network::debug_conv3(const float* h_in, int cin, Int3 size, const float* h_w
   CFB_CUDA(cudaMemcpyAsync(d_in, h_in, (size_t)cin * v * 4, cudaMemcpyHostToDevice, s));
   CFB_CUDA(cudaMemcpyAsync(d_w, h_w, (size_t)cout * cin * 27 * 4, cudaMemcpyHostToDevice, s));
   CFB_CUDA(cudaMemcpyAsync(d_b, h_b, (size_t)cout * 4, cudaMemcpyHostToDevice, s));
-  if (umma()) {
+  if (tensor_cores()) {
     if (cin % 16) { cudaFree(d_in); cudaFree(d_w); cudaFree(d_b); cudaFree(d_out); throw std::runtime_error("the wgmma convolution needs cin % 16 == 0"); }
     const int P = parts();
     __half *c_in = nullptr, *c_out = nullptr;

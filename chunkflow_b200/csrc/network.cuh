@@ -2,18 +2,21 @@
 // Owns the packed weights and the activation workspace for `batch` patches in flight and
 // dispatches each layer to the kernels of the configured precision mode.
 #pragma once
+#include <array>
 #include <map>
 #include <string>
 #include <vector>
 
+#include "chunkflow_b200.h"
 #include "common.cuh"
 #include "kernels_conv.cuh"
 
 namespace cfb {
 
+// The activations of the network; the layer table in network.cu says which step produces each one.
+enum Act : int { kIn, kE0a, kE0, kP0, kE1a, kE1, kP1, kE2a, kE2, kU1, kD1a, kD1, kU0, kD0a, kD0, kOut, kNumActs, kNoAct = -1 };
+
 struct ConvLayer {
-  std::string name;
-  int cin = 0, cout = 0;
   float* w = nullptr;     // fp32, state_dict layout
   float* bias = nullptr;  // fp32
   PackedConv packed;      // B-operand blocks for the wgmma path (3x3x3 layers, cin >= 16)
@@ -27,17 +30,12 @@ class Network {
   int cnet() const { return cnet_; }
   void release();
 
-  // Extract `nb` patches from the chunk and run the network; returns kernel launches.
-  int forward_from_chunk(const void* chunk, int in_dtype, Int3 chunk_size, const PatchPos* patches, int nb,
-                         cudaStream_t s);
-  int forward_from_host_patches(const float* h_patches, int nb, cudaStream_t s);
-  // Whole-chunk path: extract + network + crop + bump mask + accumulate into the output chunk.  On the wgmma
-  // path the head and the blend are fused into the epilogue of the last convolution.
+  // Whole-chunk path: extract + network + crop + bump mask + accumulate into the output chunk; returns kernel launches.
+  // On the tensor-core path the head and the blend are fused into the epilogue of the last convolution.
   int forward_and_blend(const void* chunk, int in_dtype, Int3 chunk_size, const PatchPos* patches, int nb, Int3 out_patch,
                         Int3 crop, const float* mask, float* out, int channels, Int3 out_size, float scale, cudaStream_t s);
-  // crop + bump mask + accumulate the last forward's outputs into the output chunk.
-  int blend(Int3 out_patch, Int3 crop, const float* mask, const PatchPos* patches, int nb, float* out,
-            int channels, Int3 out_size, float scale, cudaStream_t s);
+  // Network on `nb` fp32 patches from the host; the raw output stays on the device (crop_mask, copy_raw_output_to_host).
+  int forward_from_host_patches(const float* h_patches, int nb, cudaStream_t s);
   void crop_mask(Int3 out_patch, Int3 crop, const float* mask, int nb, float* dst, int channels, cudaStream_t s);
   float* patch_input_buffer(int nb);
   void copy_raw_output_to_host(float* h_out, cudaStream_t s);
@@ -49,15 +47,36 @@ class Network {
                   float* h_out, cudaStream_t s);
 
  private:
+  // How the network ends: head + blend in the epilogue of the last convolution, head + blend (tensor cores: one CUDA-core
+  // kernel, simt: the head, then the blend kernel), or the head into the raw output.
+  enum End { kFusedTail, kBlend, kRawOutput };
+  // Environment switches, read once per forward call, that route it through kernels which cross-check the production ones.
+  struct CrossChecks {
+    bool no_pool_fusion;  // CFB_NO_POOL_FUSION: the (1,2,2) max pools as kernels of their own
+    bool simt_convt;      // CFB_SIMT_CONVT: the transposed convolutions on CUDA cores
+    bool no_fused_tail;   // CFB_NO_FUSED_TAIL: the head + blend as a kernel of its own
+  };
+  static CrossChecks read_cross_checks();
+  struct Route {
+    const void* chunk;  // the first layer reads the patches blend.patches from this chunk, or (nullptr) the staged fp32 patches
+    int in_dtype;
+    Int3 chunk_size;
+    End end;
+    ConvTail blend;     // the output of the blending ends; run fills in the head
+    CrossChecks checks;
+  };
+  // Issues every step of the layer table for `nb` patches with the kernels of the configured mode; returns the launches.
+  int run(const Route& r, int nb, cudaStream_t s);
+
   void allocate();
-  int forward(int nb, cudaStream_t s);  // from buf_in_ (fp32 SIMT path)
-  // wgmma path: chunk != nullptr -> first layer reads the chunk, else the staged fp32 patches in buf_in_
-  int forward_cp8(const void* chunk, int in_dtype, Int3 chunk_size, const PatchPos* patches, int nb, cudaStream_t s,
-                  bool with_head, const ConvTail* tail = nullptr);
-  bool umma() const { return precision_ != 0; }
-  // activation number format of the wgmma path (act_format.cuh) and its planes per 8-channel chunk
-  int fmt() const { return precision_ == 1 ? kFmtF16x2 : (precision_ == 3 ? kFmtF16F8 : kFmtF16); }
+  bool tensor_cores() const { return precision_ != CFB_PRECISION_F32_SIMT; }
+  // activation number format of the tensor-core path (act_format.cuh) and its planes per 8-channel chunk
+  int fmt() const {
+    return precision_ == CFB_PRECISION_F16X3_UMMA ? kFmtF16x2 : precision_ == CFB_PRECISION_F16F8_UMMA ? kFmtF16F8 : kFmtF16;
+  }
   int parts() const { return fmt_planes(fmt()); }
+  float* f32(Act a) const { return static_cast<float*>(act_[a]); }
+  __half* cp8(Act a) const { return static_cast<__half*>(act_[a]); }
 
   struct Span { int id; cudaEvent_t a, b; };
   void prof_begin(const char* name, cudaStream_t s);
@@ -75,17 +94,11 @@ class Network {
   int batch_ = 1;
   bool ready_ = false;
   int cnet_ = 0;
-  FirstConvW first_w_{};  // host copy of the first layer, passed to its kernel by value
-  std::map<std::string, ConvLayer> layers_;
+  FirstConvW first_w_{};              // host copy of the first layer, passed to its kernel by value
+  std::vector<ConvLayer> layers_;     // by index into the layer table
   std::vector<void*> owned_;
-  // fp32 planar activations, (batch, C, Z, Y, X)
-  float *buf_in_ = nullptr, *e0a_ = nullptr, *e0_ = nullptr, *p0_ = nullptr, *e1a_ = nullptr, *e1_ = nullptr,
-        *p1_ = nullptr, *e2a_ = nullptr, *e2_ = nullptr, *u1_ = nullptr, *d1a_ = nullptr, *d1_ = nullptr,
-        *u0_ = nullptr, *d0a_ = nullptr, *d0_ = nullptr, *net_out_ = nullptr;
-  // CP8 fp16 activations of the wgmma path
-  __half *h_e0a_ = nullptr, *h_e0_ = nullptr, *h_p0_ = nullptr, *h_e1a_ = nullptr, *h_e1_ = nullptr, *h_p1_ = nullptr,
-         *h_e2a_ = nullptr, *h_e2_ = nullptr, *h_u1_ = nullptr, *h_d1a_ = nullptr, *h_d1_ = nullptr, *h_u0_ = nullptr,
-         *h_d0a_ = nullptr, *h_d0_ = nullptr;
+  // (batch, C, Z, Y, X) fp32 for kIn, kOut and every activation of the simt mode, CP8 for the tensor-core modes
+  std::array<void*, kNumActs> act_{};
 };
 
 }  // namespace cfb

@@ -498,9 +498,9 @@ def test_host_plugin_shape_errors_and_myelin_zero_threshold():
 
 
 def test_kernel_variants_agree(monkeypatch, unet_model):
-    """Every kernel variant computes the same network: fused vs unfused head+blend tail, first layer with its weights in the constant
-    bank vs in shared memory, 3x3x3 convolutions split into z blocks, weights streamed through a ring, pooling fused into the
-    convolution epilogue vs its own kernel, tensor-core vs CUDA-core transposed convolutions (forced through env switches)."""
+    """Every kernel variant computes the same network: fused vs unfused head+blend tail, 3x3x3 convolutions split into z blocks,
+    weights streamed through a ring, pooling fused into the convolution epilogue vs its own kernel, tensor-core vs CUDA-core
+    transposed convolutions (forced through env switches)."""
     rng = np.random.default_rng(31)
     img = rng.integers(0, 256, size=(20, 96, 104), dtype=np.uint8)
     kw = dict(input_patch_size=(16, 64, 64), output_patch_overlap=(4, 16, 16), num_output_channels=3, framework="b200",
@@ -508,12 +508,10 @@ def test_kernel_variants_agree(monkeypatch, unet_model):
     ref, _ = O.infer_chunk(img, input_patch_size=(16, 64, 64), output_patch_overlap=(4, 16, 16), num_output_channels=3,
                            framework="pytorch", model=unet_model)
     results = {}
-    for name, env in [("default", {}), ("unfused_tail", {"CFB_NO_FUSED_TAIL": "1"}), ("smem_first", {"CFB_FIRST_CONV_SMEM_W": "1"}),
-                      ("zblock4", {"CFB_FORCE_ZBLOCK": "4"}), ("weight_ring", {"CFB_FORCE_WEIGHT_RING": "1"}),
-                      ("zblock2_ring", {"CFB_FORCE_ZBLOCK": "2", "CFB_FORCE_WEIGHT_RING": "1"}),
+    for name, env in [("default", {}), ("unfused_tail", {"CFB_NO_FUSED_TAIL": "1"}), ("zblock4", {"CFB_FORCE_ZBLOCK": "4"}),
+                      ("weight_ring", {"CFB_FORCE_WEIGHT_RING": "1"}), ("zblock2_ring", {"CFB_FORCE_ZBLOCK": "2", "CFB_FORCE_WEIGHT_RING": "1"}),
                       ("unfused_pool", {"CFB_NO_POOL_FUSION": "1"}), ("simt_convT", {"CFB_SIMT_CONVT": "1"})]:
-        for k in ("CFB_NO_FUSED_TAIL", "CFB_FIRST_CONV_SMEM_W", "CFB_FORCE_ZBLOCK", "CFB_FORCE_WEIGHT_RING", "CFB_NO_POOL_FUSION",
-                  "CFB_SIMT_CONVT"):
+        for k in ("CFB_NO_FUSED_TAIL", "CFB_FORCE_ZBLOCK", "CFB_FORCE_WEIGHT_RING", "CFB_NO_POOL_FUSION", "CFB_SIMT_CONVT"):
             monkeypatch.delenv(k, raising=False)
         for k, v in env.items():
             monkeypatch.setenv(k, v)
@@ -527,17 +525,16 @@ def test_kernel_variants_agree(monkeypatch, unet_model):
 
 def test_f16f8_unfused_and_cuda_core_paths(monkeypatch, unet_model):
     """The default f16f8 number format through the kernels that are not on the default route: the unfused head+blend tail, the
-    first layer with shared-memory weights, the stand-alone pool and the CUDA-core transposed convolution (they decode / encode the
-    H + A8 + L8 records through load8 / store8, kernels_cp8.cu)."""
+    stand-alone pool and the CUDA-core transposed convolution (they decode / encode the H + A8 + L8 records through load8 / store8,
+    kernels_cp8.cu)."""
     rng = np.random.default_rng(41)
     img = rng.integers(0, 256, size=(20, 96, 104), dtype=np.uint8)
     kw = dict(input_patch_size=(16, 64, 64), output_patch_overlap=(4, 16, 16), num_output_channels=3, framework="b200", batch_size=5)
     ref, _ = O.infer_chunk(img, input_patch_size=(16, 64, 64), output_patch_overlap=(4, 16, 16), num_output_channels=3,
                            framework="pytorch", model=unet_model)
-    for env in ({}, {"CFB_NO_FUSED_TAIL": "1"}, {"CFB_FIRST_CONV_SMEM_W": "1"}, {"CFB_FORCE_ZBLOCK": "2"}, {"CFB_FORCE_WEIGHT_RING": "1"},
-                {"CFB_NO_POOL_FUSION": "1"}, {"CFB_SIMT_CONVT": "1"}):
-        for k in ("CFB_NO_FUSED_TAIL", "CFB_FIRST_CONV_SMEM_W", "CFB_FORCE_ZBLOCK", "CFB_FORCE_WEIGHT_RING", "CFB_NO_POOL_FUSION",
-                  "CFB_SIMT_CONVT"):
+    for env in ({}, {"CFB_NO_FUSED_TAIL": "1"}, {"CFB_FORCE_ZBLOCK": "2"}, {"CFB_FORCE_WEIGHT_RING": "1"}, {"CFB_NO_POOL_FUSION": "1"},
+                {"CFB_SIMT_CONVT": "1"}):
+        for k in ("CFB_NO_FUSED_TAIL", "CFB_FORCE_ZBLOCK", "CFB_FORCE_WEIGHT_RING", "CFB_NO_POOL_FUSION", "CFB_SIMT_CONVT"):
             monkeypatch.delenv(k, raising=False)
         for k, v in env.items():
             monkeypatch.setenv(k, v)
