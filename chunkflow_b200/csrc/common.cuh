@@ -5,6 +5,9 @@
 #include <cstdio>
 #include <stdexcept>
 #include <string>
+#include <utility>
+
+#include "chunkflow_b200.h"
 
 namespace cfb {
 
@@ -30,6 +33,57 @@ struct CudaError : std::runtime_error {
   } while (0)
 
 #define CFB_LAUNCH_CHECK() CFB_CUDA(cudaGetLastError())
+
+// The error boundary of every C-ABI entry point: an exception becomes a status code, its message cfb_last_error().
+template <typename F>
+int guarded(F&& f) {
+  try {
+    return f();
+  } catch (const std::invalid_argument& ex) {
+    set_last_error(ex.what());
+    return CFB_ERR_INVALID_ARGUMENT;
+  } catch (const CudaError& ex) {
+    set_last_error(ex.what());
+    return CFB_ERR_CUDA;
+  } catch (const std::exception& ex) {
+    set_last_error(ex.what());
+    return CFB_ERR_UNSUPPORTED;
+  }
+}
+
+// One device allocation, freed with its owner (on the device current at that time).
+class DeviceBuffer {
+ public:
+  DeviceBuffer() = default;
+  explicit DeviceBuffer(size_t bytes) { grow(bytes); }
+  DeviceBuffer(DeviceBuffer&& o) noexcept : p_(std::exchange(o.p_, nullptr)), bytes_(std::exchange(o.bytes_, 0)) {}
+  DeviceBuffer& operator=(DeviceBuffer&& o) noexcept {
+    std::swap(p_, o.p_);
+    std::swap(bytes_, o.bytes_);
+    return *this;
+  }
+  ~DeviceBuffer() { reset(); }
+
+  // Makes the buffer at least `bytes` long; a new allocation does not keep the contents.
+  void grow(size_t bytes) {
+    if (p_ && bytes <= bytes_) return;
+    reset();
+    CFB_CUDA(cudaMalloc(&p_, bytes));
+    bytes_ = bytes;
+  }
+  void reset() {
+    if (p_) cudaFree(p_);  // unchecked: also runs in destructors
+    p_ = nullptr;
+    bytes_ = 0;
+  }
+  template <typename T = void>
+  T* as() const { return static_cast<T*>(p_); }
+  explicit operator bool() const { return p_ != nullptr; }
+
+ private:
+  void* p_ = nullptr;
+  size_t bytes_ = 0;
+};
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline int64_t ceil_div64(int64_t a, int64_t b) { return (a + b - 1) / b; }

@@ -87,6 +87,13 @@ static AxisGrid axis_grid(int size, int ip, int ioverlap, int istride, int pcrop
   return g;
 }
 
+// The patch grid on one chunk shape (reference inferencer.py:183-204,255-292).
+struct ChunkGeometry {
+  Int3 size{0, 0, 0};  // the input chunk
+  Int3 out{0, 0, 0};   // the output buffer: the chunk less the output crop margin on either side
+  AxisGrid z, y, x;
+};
+
 }  // namespace cfb
 
 using namespace cfb;
@@ -98,29 +105,22 @@ struct cfb_engine {
   std::map<std::string, std::vector<float>> host_w;
   Network net;
   std::vector<float> h_mask;
-  float* d_mask = nullptr;
+  DeviceBuffer mask;
 
-  // per-chunk-shape cache (the reference caches its output_chunk_mask the same way, :300-312)
-  Int3 cached_chunk{0, 0, 0};
-  Int3 out_size{0, 0, 0};
-  AxisGrid gz, gy, gx;
+  // per-chunk-shape cache (prepare_chunk; the reference caches its output_chunk_mask the same way, :300-312)
+  ChunkGeometry geo;
   std::vector<PatchPos> h_patches;
-  PatchPos* d_patches = nullptr;
-  int* d_cover = nullptr;  // cover_z | cover_y | cover_x | oz0 | oy0 | ox0
-  int *d_cover_z = nullptr, *d_cover_y = nullptr, *d_cover_x = nullptr, *d_oz0 = nullptr, *d_oy0 = nullptr, *d_ox0 = nullptr;
-  float* d_winv = nullptr;
-  bool winv_valid = false;
-  int* d_cover_z_slab = nullptr;
-  size_t cover_z_slab_cap = 0;
+  DeviceBuffer patches;
+  DeviceBuffer cover_tables;  // `cover` points into it
+  CoverTables cover{};
+  DeviceBuffer winv;          // 1/W of `geo`, computed on first use (inverse_weight)
+  DeviceBuffer slab_cover_tables;
 
-  unsigned int* d_flags = nullptr;  // [0] nonzero flag, [1] max bits
+  DeviceBuffer flags;  // unsigned int [0] nonzero flag, [1] max bits
   cudaStream_t own_stream = nullptr;
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t ev_ready = nullptr;
-  void* d_host_in = nullptr; size_t host_in_cap = 0;
-  float* d_host_out = nullptr; size_t host_out_cap = 0;
-  float* d_plugin_out = nullptr; size_t plugin_out_cap = 0;
-  float* d_plugin_in = nullptr; size_t plugin_in_cap = 0;
+  DeviceBuffer host_in, host_out, plugin_out, plugin_in;
   bool plugin_active = false; int plugin_dtype = 0;
 
   std::unique_ptr<HostStager> stager;  // pinned ring + host threads for results that go to pageable memory
@@ -139,12 +139,24 @@ struct cfb_engine {
   int variant_flags(int v) const { return (p.augment == CFB_AUGMENT_REFERENCE && variants() > 1) ? (v | kTtaChannelSym) : v; }
   float variant_scale() const { return variants() == 1 ? 1.0f : (p.augment == CFB_AUGMENT_SPATIAL ? 0.125f : 0.25f); }
 
+  // Every entry point that takes a chunk shape checks it here, in this order.
+  ChunkGeometry geometry(int64_t cz, int64_t cy, int64_t cx) const {
+    if (cz < ip.z || cy < ip.y || cx < ip.x) throw std::invalid_argument("input chunk is smaller than the input patch");
+    if (cz > INT32_MAX || cy > INT32_MAX || cx > INT32_MAX) throw std::invalid_argument("chunk too large");
+    ChunkGeometry g;
+    g.size = Int3{(int)cz, (int)cy, (int)cx};
+    g.out = Int3{g.size.z - 2 * ocm.z, g.size.y - 2 * ocm.y, g.size.x - 2 * ocm.x};  // inferencer.py:194-196
+    if (g.out.z <= 0 || g.out.y <= 0 || g.out.x <= 0) throw std::invalid_argument("output crop margin swallows the chunk");
+    g.z = axis_grid(g.size.z, ip.z, ioverlap.z, istride.z, pcrop.z, ocm.z);
+    g.y = axis_grid(g.size.y, ip.y, ioverlap.y, istride.y, pcrop.y, ocm.y);
+    g.x = axis_grid(g.size.x, ip.x, ioverlap.x, istride.x, pcrop.x, ocm.x);
+    return g;
+  }
+
   ~cfb_engine() {
-    cudaSetDevice(p.device);
+    cudaSetDevice(p.device);  // the DeviceBuffer members are freed after this body, on this device
     stager.reset();
     net.release();
-    cudaFree(d_mask); cudaFree(d_patches); cudaFree(d_cover); cudaFree(d_winv); cudaFree(d_flags);
-    cudaFree(d_cover_z_slab); cudaFree(d_host_in); cudaFree(d_host_out); cudaFree(d_plugin_out); cudaFree(d_plugin_in);
     for (auto& e : ev) if (e) cudaEventDestroy(e);
     if (own_stream) cudaStreamDestroy(own_stream);
     if (copy_stream) cudaStreamDestroy(copy_stream);
@@ -154,86 +166,113 @@ struct cfb_engine {
 
 namespace {
 
-template <typename T>
-void ensure(T*& ptr, size_t& cap, size_t bytes) {
-  if (bytes <= cap && ptr) return;
-  if (ptr) CFB_CUDA(cudaFree(ptr));
-  ptr = nullptr; cap = 0;
-  CFB_CUDA(cudaMalloc(&ptr, bytes));
-  cap = bytes;
-}
-
-void build_cover(const AxisGrid& g, int op_len, int out_len, std::vector<int>& cover, int row_begin = 0, int row_end = -1) {
-  if (row_end < 0) row_end = (int)g.out_start.size();
-  cover.assign((size_t)out_len * kMaxCover, -1);
+// Appends the cover table of one output axis, counting the patch axis-indices [row_begin, row_end): for every
+// coordinate the covering indices ascending, then -1 up to kMaxCover entries.
+void append_cover(const AxisGrid& g, int op_len, int out_len, int row_begin, int row_end, std::vector<int>& t) {
+  const size_t base = t.size();
+  t.resize(base + (size_t)out_len * kMaxCover, -1);
   for (int v = 0; v < out_len; ++v) {
     int n = 0;
     for (int k = row_begin; k < row_end; ++k) {
       if (g.out_start[k] <= v && v < g.out_start[k] + op_len) {
         if (n == kMaxCover) throw std::runtime_error("a voxel is covered by more than 4 patches along one axis (overlap too large)");
-        cover[(size_t)v * kMaxCover + n++] = k;
+        t[base + (size_t)v * kMaxCover + n++] = k;
       }
     }
   }
 }
 
-void prepare_chunk(cfb_engine* e, int64_t cz, int64_t cy, int64_t cx, cudaStream_t s) {
-  if (cz < e->ip.z || cy < e->ip.y || cx < e->ip.x)
-    throw std::invalid_argument("input chunk is smaller than the input patch");
-  if (cz > INT32_MAX || cy > INT32_MAX || cx > INT32_MAX) throw std::invalid_argument("chunk too large");
-  if (e->cached_chunk.z == cz && e->cached_chunk.y == cy && e->cached_chunk.x == cx) return;
-  e->winv_valid = false;
-  e->cached_chunk = Int3{0, 0, 0};
-  const Int3 out{(int)cz - 2 * e->ocm.z, (int)cy - 2 * e->ocm.y, (int)cx - 2 * e->ocm.x};  // inferencer.py:194-196
-  if (out.z <= 0 || out.y <= 0 || out.x <= 0) throw std::invalid_argument("output crop margin swallows the chunk");
-  e->gz = axis_grid((int)cz, e->ip.z, e->ioverlap.z, e->istride.z, e->pcrop.z, e->ocm.z);
-  e->gy = axis_grid((int)cy, e->ip.y, e->ioverlap.y, e->istride.y, e->pcrop.y, e->ocm.y);
-  e->gx = axis_grid((int)cx, e->ip.x, e->ioverlap.x, e->istride.x, e->pcrop.x, e->ocm.x);
-  e->h_patches.clear();
-  for (size_t a = 0; a < e->gz.in_start.size(); ++a)
-    for (size_t b = 0; b < e->gy.in_start.size(); ++b)
-      for (size_t c = 0; c < e->gx.in_start.size(); ++c)
-        for (int v = 0; v < e->variants(); ++v)  // 8 flip/transpose variants per patch with --augment
-          e->h_patches.push_back(PatchPos{e->gz.in_start[a], e->gy.in_start[b], e->gx.in_start[c],
-                                          e->gz.out_start[a], e->gy.out_start[b], e->gx.out_start[c], e->variant_flags(v)});
-  if (e->h_patches.empty()) throw std::invalid_argument("no patch fits the chunk");
-  cudaFree(e->d_patches); e->d_patches = nullptr;
-  CFB_CUDA(cudaMalloc(&e->d_patches, e->h_patches.size() * sizeof(PatchPos)));
-  CFB_CUDA(cudaMemcpyAsync(e->d_patches, e->h_patches.data(), e->h_patches.size() * sizeof(PatchPos),
-                           cudaMemcpyHostToDevice, s));
-  std::vector<int> cz_t, cy_t, cx_t;
-  build_cover(e->gz, e->op.z, out.z, cz_t);
-  build_cover(e->gy, e->op.y, out.y, cy_t);
-  build_cover(e->gx, e->op.x, out.x, cx_t);
-  std::vector<int> all;
-  all.insert(all.end(), cz_t.begin(), cz_t.end());
-  all.insert(all.end(), cy_t.begin(), cy_t.end());
-  all.insert(all.end(), cx_t.begin(), cx_t.end());
-  all.insert(all.end(), e->gz.out_start.begin(), e->gz.out_start.end());
-  all.insert(all.end(), e->gy.out_start.begin(), e->gy.out_start.end());
-  all.insert(all.end(), e->gx.out_start.begin(), e->gx.out_start.end());
-  cudaFree(e->d_cover); e->d_cover = nullptr;
-  CFB_CUDA(cudaMalloc(&e->d_cover, all.size() * sizeof(int)));
-  CFB_CUDA(cudaMemcpyAsync(e->d_cover, all.data(), all.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-  CFB_CUDA(cudaStreamSynchronize(s));  // host vectors above are temporaries
-  e->d_cover_z = e->d_cover;
-  e->d_cover_y = e->d_cover_z + cz_t.size();
-  e->d_cover_x = e->d_cover_y + cy_t.size();
-  e->d_oz0 = e->d_cover_x + cx_t.size();
-  e->d_oy0 = e->d_oz0 + e->gz.out_start.size();
-  e->d_ox0 = e->d_oy0 + e->gy.out_start.size();
-  cudaFree(e->d_winv); e->d_winv = nullptr;
-  e->out_size = out;
-  e->cached_chunk = Int3{(int)cz, (int)cy, (int)cx};
+// Builds the weight-volume tables of `g` in one host array, in the order of CoverTables, and uploads it into `buf`.
+// The z cover table counts the patch z-rows [row_begin, row_end) only: those of one slab.
+CoverTables upload_cover_tables(const ChunkGeometry& g, Int3 op, DeviceBuffer& buf, cudaStream_t s, int row_begin = 0,
+                                int row_end = -1) {
+  if (row_end < 0) row_end = (int)g.z.out_start.size();
+  std::vector<int> host;
+  append_cover(g.z, op.z, g.out.z, row_begin, row_end, host);
+  append_cover(g.y, op.y, g.out.y, 0, (int)g.y.out_start.size(), host);
+  append_cover(g.x, op.x, g.out.x, 0, (int)g.x.out_start.size(), host);
+  for (const AxisGrid* a : {&g.z, &g.y, &g.x}) host.insert(host.end(), a->out_start.begin(), a->out_start.end());
+  buf.grow(host.size() * sizeof(int));
+  CFB_CUDA(cudaMemcpyAsync(buf.as(), host.data(), host.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  CFB_CUDA(cudaStreamSynchronize(s));  // `host` is a temporary
+  CoverTables t;
+  t.cover_z = buf.as<int>();
+  t.cover_y = t.cover_z + (size_t)g.out.z * kMaxCover;
+  t.cover_x = t.cover_y + (size_t)g.out.y * kMaxCover;
+  t.ostart_z = t.cover_x + (size_t)g.out.x * kMaxCover;
+  t.ostart_y = t.ostart_z + g.z.out_start.size();
+  t.ostart_x = t.ostart_y + g.y.out_start.size();
+  return t;
 }
 
-void ensure_winv(cfb_engine* e, cudaStream_t s) {
-  if (e->winv_valid) return;
-  if (!e->d_winv) CFB_CUDA(cudaMalloc(&e->d_winv, vol(e->out_size) * sizeof(float)));
-  launch_weight_volume(e->d_mask, e->op, e->d_cover_z, e->d_cover_y, e->d_cover_x, e->d_oz0, e->d_oy0, e->d_ox0,
-                       e->out_size, e->d_winv, /*invert=*/true, s);
-  e->launches++;
-  e->winv_valid = true;
+void prepare_chunk(cfb_engine* e, int64_t cz, int64_t cy, int64_t cx, cudaStream_t s) {
+  ChunkGeometry g = e->geometry(cz, cy, cx);  // checked before the cache: an empty cache holds the shape (0, 0, 0)
+  if (e->geo.size.z == g.size.z && e->geo.size.y == g.size.y && e->geo.size.x == g.size.x) return;
+  e->geo = ChunkGeometry{};  // no shape is cached until its tables are on the device
+  // Freed, not reused in place: cudaFree waits for the kernels of earlier calls, on any stream, that may still read them.
+  e->winv.reset();
+  e->patches.reset();
+  e->cover_tables.reset();
+  e->h_patches.clear();
+  for (size_t a = 0; a < g.z.in_start.size(); ++a)
+    for (size_t b = 0; b < g.y.in_start.size(); ++b)
+      for (size_t c = 0; c < g.x.in_start.size(); ++c)
+        for (int v = 0; v < e->variants(); ++v)  // 8 flip/transpose variants per patch with --augment
+          e->h_patches.push_back(PatchPos{g.z.in_start[a], g.y.in_start[b], g.x.in_start[c],
+                                          g.z.out_start[a], g.y.out_start[b], g.x.out_start[c], e->variant_flags(v)});
+  const size_t bytes = e->h_patches.size() * sizeof(PatchPos);
+  e->patches.grow(bytes);
+  CFB_CUDA(cudaMemcpyAsync(e->patches.as(), e->h_patches.data(), bytes, cudaMemcpyHostToDevice, s));
+  e->cover = upload_cover_tables(g, e->op, e->cover_tables, s);
+  e->geo = std::move(g);
+}
+
+const float* inverse_weight(cfb_engine* e, cudaStream_t s) {
+  if (!e->winv) {
+    DeviceBuffer w(vol(e->geo.out) * sizeof(float));
+    launch_weight_volume(e->mask.as<float>(), e->op, e->cover, e->geo.out, w.as<float>(), /*invert=*/true, s);
+    e->launches++;
+    e->winv = std::move(w);
+  }
+  return e->winv.as<float>();
+}
+
+// a6 on an empty accumulator: clears the flags, tests the input chunk for a non-zero voxel and zeroes `out`, the output
+// buffer of `geo`.  Returns the launches.
+int start_chunk(cfb_engine* e, const void* d_in, int in_dtype, float* out, cudaStream_t s) {
+  unsigned int* flags = e->flags.as<unsigned int>();
+  CFB_CUDA(cudaMemsetAsync(flags, 0, 2 * sizeof(unsigned int), s));
+  launch_any_nonzero(d_in, in_dtype, vol(e->geo.size), flags, s);
+  CFB_CUDA(cudaMemsetAsync(out, 0, (size_t)e->p.num_output_channels * vol(e->geo.out) * sizeof(float), s));
+  return 1;
+}
+
+// a12 + a14 on a (channels, nvox) volume: out *= w (1/W, or W if !w_is_inverse; none without a weight) over `count` voxels
+// per channel from voxel `first` (count < 0: all), tracking the maximum into the flags; then the myelin mask when it is
+// configured, which needs the whole volume (the progressive download is off with it).  Returns the launches.
+int finish_output(cfb_engine* e, float* out, const float* w, bool w_is_inverse, int channels, int64_t nvox, cudaStream_t s,
+                  int64_t first = 0, int64_t count = -1) {
+  if (e->p.has_myelin_threshold && count >= 0) throw std::logic_error("the myelin mask needs the whole output volume");
+  unsigned int* flags = e->flags.as<unsigned int>();
+  launch_normalize(out + first, w ? w + first : nullptr, w_is_inverse, channels, count < 0 ? nvox : count, flags + 1, flags, s,
+                   nvox);
+  if (!e->p.has_myelin_threshold) return 1;
+  launch_myelin_mask(out, channels, nvox, e->p.mask_myelin_threshold, s);
+  return 2;
+}
+
+// a13 (reference inferencer.py:465-466) when check_output_range is set: reads the maximum the normalisation tracked, which
+// synchronises `s`.
+int output_range_status(cfb_engine* e, cudaStream_t s) {
+  if (!e->p.check_output_range) return CFB_OK;
+  unsigned int flags[2];
+  CFB_CUDA(cudaMemcpyAsync(flags, e->flags.as(), sizeof(flags), cudaMemcpyDeviceToHost, s));
+  CFB_CUDA(cudaStreamSynchronize(s));
+  float vmax;
+  std::memcpy(&vmax, &flags[1], 4);
+  if (vmax < 1.0001f) return CFB_OK;
+  set_last_error("output buffer should not be greater than 1 (max = " + std::to_string(vmax) + ")");
+  return CFB_ERR_OUTPUT_RANGE;
 }
 
 // Progressive download (host variant): output planes are final as soon as every patch z-row that
@@ -257,10 +296,9 @@ bool is_pinned_host(const void* p) {
 void flush_planes(cfb_engine* e, Progressive* pg, float* d_out, int z_end, cudaStream_t s) {
   if (z_end <= pg->planes_done) return;
   const int C = e->p.num_output_channels;
-  const int64_t plane = (int64_t)e->out_size.y * e->out_size.x, nvox = vol(e->out_size);
+  const int64_t plane = (int64_t)e->geo.out.y * e->geo.out.x, nvox = vol(e->geo.out);
   const int64_t off = (int64_t)pg->planes_done * plane, count = (int64_t)(z_end - pg->planes_done) * plane;
-  launch_normalize(d_out + off, pg->winv ? pg->winv + off : nullptr, true, C, count, e->d_flags + 1, e->d_flags, s, nvox);
-  e->launches++;
+  e->launches += finish_output(e, d_out, pg->winv, true, C, nvox, s, off, count);
   if (pg->stager) {
     for (int c = 0; c < C; ++c)
       pg->stager->push(d_out + c * nvox + off, pg->h_out + c * nvox + off, (size_t)count * sizeof(float), s, pg->copy_stream);
@@ -277,24 +315,25 @@ void flush_planes(cfb_engine* e, Progressive* pg, float* d_out, int z_end, cudaS
 // Runs the patch loop for patches [first, last) and accumulates into d_out.
 void run_patches(cfb_engine* e, const void* d_in, int in_dtype, int64_t first, int64_t last, float* d_out,
                  cudaStream_t s, Progressive* pg = nullptr) {
-  const Int3 cs = e->cached_chunk;
+  const ChunkGeometry& g = e->geo;
   const int C = e->p.num_output_channels;
   const int B = std::max(1, e->p.batch_size);
-  const int64_t per_row = (int64_t)e->gy.in_start.size() * e->gx.in_start.size() * e->variants();
+  const int64_t per_row = (int64_t)g.y.in_start.size() * g.x.in_start.size() * e->variants();
   const float scale = e->variant_scale();
   for (int64_t i = first; i < last; i += B) {
     const int nb = (int)std::min<int64_t>(B, last - i);
     if (pg) {
       // every patch of z-rows < row is launched: planes below the output start of `row` are final
       const int64_t row = i / per_row;
-      if (row < (int64_t)e->gz.out_start.size()) flush_planes(e, pg, d_out, std::max(0, std::min(e->gz.out_start[row], e->out_size.z)), s);
+      if (row < (int64_t)g.z.out_start.size()) flush_planes(e, pg, d_out, std::max(0, std::min(g.z.out_start[row], g.out.z)), s);
     }
-    const PatchPos* pp = e->d_patches + i;
+    const PatchPos* pp = e->patches.as<PatchPos>() + i;
     if (e->p.framework == CFB_FRAMEWORK_IDENTITY) {
-      launch_identity_blend(d_in, in_dtype, cs, e->ip, e->op, e->pcrop, e->d_mask, pp, nb, d_out, C, e->out_size, s);
+      launch_identity_blend(d_in, in_dtype, g.size, e->ip, e->op, e->pcrop, e->mask.as<float>(), pp, nb, d_out, C, g.out, s);
       e->launches++;
     } else {
-      e->launches += e->net.forward_and_blend(d_in, in_dtype, cs, pp, nb, e->op, e->pcrop, e->d_mask, d_out, C, e->out_size, scale, s);
+      e->launches += e->net.forward_and_blend(d_in, in_dtype, g.size, pp, nb, e->op, e->pcrop, e->mask.as<float>(), d_out, C, g.out,
+                                              scale, s);
     }
   }
 }
@@ -311,13 +350,8 @@ int infer_impl(cfb_engine* e, const void* d_in, int in_dtype, int64_t cz, int64_
   e->launches = 0;
   CFB_CUDA(cudaEventRecord(e->ev[0], s));
   prepare_chunk(e, cz, cy, cx, s);
-  const int C = e->p.num_output_channels;
-  const int64_t nvox = vol(e->out_size);
-  CFB_CUDA(cudaMemsetAsync(e->d_flags, 0, 2 * sizeof(unsigned int), s));
-  launch_any_nonzero(d_in, in_dtype, cz * cy * cx, e->d_flags, s);
-  e->launches++;
-  CFB_CUDA(cudaMemsetAsync(d_out, 0, (size_t)C * nvox * sizeof(float), s));
-  const int64_t ny = e->gy.in_start.size(), nx = e->gx.in_start.size(), nz = e->gz.in_start.size();
+  e->launches += start_chunk(e, d_in, in_dtype, d_out, s);
+  const int64_t ny = e->geo.y.in_start.size(), nx = e->geo.x.in_start.size(), nz = e->geo.z.in_start.size();
   if (slab) {
     if (zrow_begin < 0 || zrow_end > nz || zrow_begin > zrow_end) throw std::invalid_argument("bad z-row range");
   } else {
@@ -325,64 +359,27 @@ int infer_impl(cfb_engine* e, const void* d_in, int in_dtype, int64_t cz, int64_
   }
   if (pg) {
     if (slab || e->p.has_myelin_threshold) pg = nullptr;  // those need the whole volume before the final pass
-    else if (e->p.mask_output_chunk) { ensure_winv(e, s); pg->winv = e->d_winv; }
+    else if (e->p.mask_output_chunk) pg->winv = inverse_weight(e, s);
   }
   CFB_CUDA(cudaEventRecord(e->ev[1], s));
   run_patches(e, d_in, in_dtype, zrow_begin * ny * nx * e->variants(), zrow_end * ny * nx * e->variants(), d_out, s, pg);
   CFB_CUDA(cudaEventRecord(e->ev[2], s));
   if (slab && d_weight) {
     // partial weight sum of this slab's patches only
-    std::vector<int> cz_t;
-    build_cover(e->gz, e->op.z, e->out_size.z, cz_t, (int)zrow_begin, (int)zrow_end);
-    ensure(e->d_cover_z_slab, e->cover_z_slab_cap, cz_t.size() * sizeof(int));
-    CFB_CUDA(cudaMemcpyAsync(e->d_cover_z_slab, cz_t.data(), cz_t.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-    CFB_CUDA(cudaStreamSynchronize(s));
-    launch_weight_volume(e->d_mask, e->op, e->d_cover_z_slab, e->d_cover_y, e->d_cover_x, e->d_oz0, e->d_oy0,
-                         e->d_ox0, e->out_size, d_weight, /*invert=*/false, s);
+    const CoverTables t = upload_cover_tables(e->geo, e->op, e->slab_cover_tables, s, (int)zrow_begin, (int)zrow_end);
+    launch_weight_volume(e->mask.as<float>(), e->op, t, e->geo.out, d_weight, /*invert=*/false, s);
     e->launches++;
   } else if (slab) {
     // no partial weight volume wanted: the owner of a plane computes the full weight sum itself (cfb_weight_volume_device)
   } else if (pg) {
-    flush_planes(e, pg, d_out, e->out_size.z, s);  // remaining planes
+    flush_planes(e, pg, d_out, e->geo.out.z, s);  // remaining planes
   } else {
-    const float* w = nullptr;
-    if (e->p.mask_output_chunk) { ensure_winv(e, s); w = e->d_winv; }
-    launch_normalize(d_out, w, true, C, nvox, e->d_flags + 1, e->d_flags, s);
-    e->launches++;
-    if (e->p.has_myelin_threshold) {
-      launch_myelin_mask(d_out, C, nvox, e->p.mask_myelin_threshold, s);
-      e->launches++;
-    }
+    const float* w = e->p.mask_output_chunk ? inverse_weight(e, s) : nullptr;
+    e->launches += finish_output(e, d_out, w, true, e->p.num_output_channels, vol(e->geo.out), s);
   }
   CFB_CUDA(cudaEventRecord(e->ev[3], s));
   e->timing_valid = true;
-  if (!slab && e->p.check_output_range) {
-    unsigned int flags[2];
-    CFB_CUDA(cudaMemcpyAsync(flags, e->d_flags, sizeof(flags), cudaMemcpyDeviceToHost, s));
-    CFB_CUDA(cudaStreamSynchronize(s));
-    float vmax; std::memcpy(&vmax, &flags[1], 4);
-    if (!(vmax < 1.0001f)) {  // reference inferencer.py:465-466
-      set_last_error("output buffer should not be greater than 1 (max = " + std::to_string(vmax) + ")");
-      return CFB_ERR_OUTPUT_RANGE;
-    }
-  }
-  return CFB_OK;
-}
-
-template <typename F>
-int guarded(F&& f) {
-  try {
-    return f();
-  } catch (const std::invalid_argument& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_INVALID_ARGUMENT;
-  } catch (const CudaError& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_CUDA;
-  } catch (const std::exception& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_UNSUPPORTED;
-  }
+  return slab ? CFB_OK : output_range_status(e, s);
 }
 
 }  // namespace
@@ -455,9 +452,9 @@ int cfb_create(const cfb_params* params, cfb_handle* out) {
       return CFB_ERR_CUDA;
     }
     e->h_mask = build_patch_mask(e->op, e->ovl);
-    CFB_CUDA(cudaMalloc(&e->d_mask, e->h_mask.size() * sizeof(float)));
-    CFB_CUDA(cudaMemcpy(e->d_mask, e->h_mask.data(), e->h_mask.size() * sizeof(float), cudaMemcpyHostToDevice));
-    CFB_CUDA(cudaMalloc(&e->d_flags, 2 * sizeof(unsigned int)));
+    e->mask.grow(e->h_mask.size() * sizeof(float));
+    CFB_CUDA(cudaMemcpy(e->mask.as(), e->h_mask.data(), e->h_mask.size() * sizeof(float), cudaMemcpyHostToDevice));
+    e->flags.grow(2 * sizeof(unsigned int));
     CFB_CUDA(cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking));
     CFB_CUDA(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
     CFB_CUDA(cudaEventCreateWithFlags(&e->ev_ready, cudaEventDisableTiming));
@@ -508,14 +505,11 @@ int cfb_patch_grid(cfb_handle h, int64_t cz, int64_t cy, int64_t cx, int64_t* nu
                    int64_t capacity) {
   return guarded([&]() -> int {
     if (!h || !num_patches) throw std::invalid_argument("null argument");
-    if (cz < h->ip.z || cy < h->ip.y || cx < h->ip.x) throw std::invalid_argument("input chunk is smaller than the input patch");
-    AxisGrid gz = axis_grid((int)cz, h->ip.z, h->ioverlap.z, h->istride.z, h->pcrop.z, h->ocm.z);
-    AxisGrid gy = axis_grid((int)cy, h->ip.y, h->ioverlap.y, h->istride.y, h->pcrop.y, h->ocm.y);
-    AxisGrid gx = axis_grid((int)cx, h->ip.x, h->ioverlap.x, h->istride.x, h->pcrop.x, h->ocm.x);
-    *num_patches = (int64_t)gz.in_start.size() * gy.in_start.size() * gx.in_start.size();
+    const ChunkGeometry g = h->geometry(cz, cy, cx);
+    *num_patches = (int64_t)g.z.in_start.size() * g.y.in_start.size() * g.x.in_start.size();
     if (starts_zyx) {
       int64_t k = 0;
-      for (int a : gz.in_start) for (int b : gy.in_start) for (int c : gx.in_start) {
+      for (int a : g.z.in_start) for (int b : g.y.in_start) for (int c : g.x.in_start) {
         if (k >= capacity) return CFB_OK;
         starts_zyx[3 * k] = a; starts_zyx[3 * k + 1] = b; starts_zyx[3 * k + 2] = c; ++k;
       }
@@ -527,9 +521,9 @@ int cfb_patch_grid(cfb_handle h, int64_t cz, int64_t cy, int64_t cx, int64_t* nu
 int cfb_output_shape(cfb_handle h, int64_t cz, int64_t cy, int64_t cx, int64_t out_czyx[4]) {
   return guarded([&]() -> int {
     if (!h || !out_czyx) throw std::invalid_argument("null argument");
+    const Int3 out = h->geometry(cz, cy, cx).out;
     out_czyx[0] = h->p.num_output_channels;
-    out_czyx[1] = cz - 2 * h->ocm.z; out_czyx[2] = cy - 2 * h->ocm.y; out_czyx[3] = cx - 2 * h->ocm.x;
-    if (out_czyx[1] <= 0 || out_czyx[2] <= 0 || out_czyx[3] <= 0) throw std::invalid_argument("output crop margin swallows the chunk");
+    out_czyx[1] = out.z; out_czyx[2] = out.y; out_czyx[3] = out.x;
     return CFB_OK;
   });
 }
@@ -556,22 +550,11 @@ int cfb_normalize_device(cfb_handle h, float* d_out, const float* d_weight, int3
     if (!h || !d_out) throw std::invalid_argument("null argument");
     CFB_CUDA(cudaSetDevice(h->p.device));
     cudaStream_t s = (cudaStream_t)stream;
-    // d_flags[0]: the nonzero flag the kernel reads (0 forces the output to zero, reference inferencer.py:387-393)
+    // flags[0]: the nonzero flag the kernel reads (0 forces the output to zero, reference inferencer.py:387-393)
     const unsigned int init[2] = {all_zero_input ? 0u : 1u, 0u};
-    CFB_CUDA(cudaMemcpyAsync(h->d_flags, init, sizeof(init), cudaMemcpyHostToDevice, s));
-    launch_normalize(d_out, d_weight, weight_is_inverse != 0, (int)channels, oz * oy * ox, h->d_flags + 1, h->d_flags, s);
-    if (h->p.has_myelin_threshold) launch_myelin_mask(d_out, (int)channels, oz * oy * ox, h->p.mask_myelin_threshold, s);
-    if (h->p.check_output_range) {
-      unsigned int flags[2];
-      CFB_CUDA(cudaMemcpyAsync(flags, h->d_flags, sizeof(flags), cudaMemcpyDeviceToHost, s));
-      CFB_CUDA(cudaStreamSynchronize(s));
-      float vmax; std::memcpy(&vmax, &flags[1], 4);
-      if (!(vmax < 1.0001f)) {  // reference inferencer.py:465-466
-        set_last_error("output buffer should not be greater than 1 (max = " + std::to_string(vmax) + ")");
-        return CFB_ERR_OUTPUT_RANGE;
-      }
-    }
-    return CFB_OK;
+    CFB_CUDA(cudaMemcpyAsync(h->flags.as(), init, sizeof(init), cudaMemcpyHostToDevice, s));
+    finish_output(h, d_out, d_weight, weight_is_inverse != 0, (int)channels, oz * oy * ox, s);
+    return output_range_status(h, s);
   });
 }
 
@@ -580,7 +563,7 @@ int cfb_slab_nonzero(cfb_handle h, int32_t* nonzero, void* stream) {
     if (!h || !nonzero) throw std::invalid_argument("null argument");
     CFB_CUDA(cudaSetDevice(h->p.device));
     unsigned int flag = 0;
-    CFB_CUDA(cudaMemcpyAsync(&flag, h->d_flags, sizeof(flag), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+    CFB_CUDA(cudaMemcpyAsync(&flag, h->flags.as(), sizeof(flag), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
     CFB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
     *nonzero = flag != 0u;
     return CFB_OK;
@@ -601,31 +584,12 @@ int cfb_weight_volume_device(cfb_handle h, int64_t cz, int64_t cy, int64_t cx, i
     if (!h || !d_weight) throw std::invalid_argument("null argument");
     CFB_CUDA(cudaSetDevice(h->p.device));
     cudaStream_t s = (cudaStream_t)stream;
-    if (cz < h->ip.z || cy < h->ip.y || cx < h->ip.x) throw std::invalid_argument("input chunk is smaller than the input patch");
-    const Int3 out{(int)cz - 2 * h->ocm.z, (int)cy - 2 * h->ocm.y, (int)cx - 2 * h->ocm.x};
-    if (z_begin < 0 || z_end > out.z || z_begin > z_end) throw std::invalid_argument("bad plane range");
-    const AxisGrid gz = axis_grid((int)cz, h->ip.z, h->ioverlap.z, h->istride.z, h->pcrop.z, h->ocm.z);
-    const AxisGrid gy = axis_grid((int)cy, h->ip.y, h->ioverlap.y, h->istride.y, h->pcrop.y, h->ocm.y);
-    const AxisGrid gx = axis_grid((int)cx, h->ip.x, h->ioverlap.x, h->istride.x, h->pcrop.x, h->ocm.x);
-    std::vector<int> tz, ty, tx, all;
-    build_cover(gz, h->op.z, out.z, tz);
-    build_cover(gy, h->op.y, out.y, ty);
-    build_cover(gx, h->op.x, out.x, tx);
-    for (const std::vector<int>* v : std::initializer_list<const std::vector<int>*>{&tz, &ty, &tx, &gz.out_start, &gy.out_start, &gx.out_start})
-      all.insert(all.end(), v->begin(), v->end());
-    int* d_tab = nullptr;
-    CFB_CUDA(cudaMalloc(&d_tab, all.size() * sizeof(int)));
-    cudaError_t err = cudaMemcpyAsync(d_tab, all.data(), all.size() * sizeof(int), cudaMemcpyHostToDevice, s);
-    if (err == cudaSuccess) {
-      const int* cz_t = d_tab; const int* cy_t = cz_t + tz.size(); const int* cx_t = cy_t + ty.size();
-      const int* oz0 = cx_t + tx.size(); const int* oy0 = oz0 + gz.out_start.size(); const int* ox0 = oy0 + gy.out_start.size();
-      try {
-        launch_weight_volume(h->d_mask, h->op, cz_t, cy_t, cx_t, oz0, oy0, ox0, out, d_weight, invert != 0, s, (int)z_begin, (int)z_end);
-      } catch (...) { cudaStreamSynchronize(s); cudaFree(d_tab); throw; }
-      err = cudaStreamSynchronize(s);  // the tables are temporaries
-    }
-    cudaFree(d_tab);
-    CFB_CUDA(err);
+    const ChunkGeometry g = h->geometry(cz, cy, cx);
+    if (z_begin < 0 || z_end > g.out.z || z_begin > z_end) throw std::invalid_argument("bad plane range");
+    DeviceBuffer tables;
+    launch_weight_volume(h->mask.as<float>(), h->op, upload_cover_tables(g, h->op, tables, s), g.out, d_weight, invert != 0, s,
+                         (int)z_begin, (int)z_end);
+    CFB_CUDA(cudaStreamSynchronize(s));  // the tables are a temporary
     return CFB_OK;
   });
 }
@@ -640,8 +604,10 @@ int cfb_infer_chunk_host(cfb_handle h, const void* h_in, int32_t in_dtype, int64
     if (rc != CFB_OK) return rc;
     const size_t in_bytes = (size_t)cz * cy * cx * (in_dtype == CFB_DTYPE_U8 ? 1 : 4);
     const size_t out_bytes = (size_t)shape[0] * shape[1] * shape[2] * shape[3] * sizeof(float);
-    ensure(h->d_host_in, h->host_in_cap, in_bytes);
-    ensure(h->d_host_out, h->host_out_cap, out_bytes);
+    h->host_in.grow(in_bytes);
+    h->host_out.grow(out_bytes);
+    void* d_in = h->host_in.as();
+    float* d_out = h->host_out.as<float>();
     cudaStream_t s = h->own_stream;
     // host arrays in pageable memory (what a drop-in caller has: plain numpy) move through the engine's own pinned ring,
     // copied by host threads; CFB_NO_HOST_STAGING=1 leaves the staging to the driver
@@ -649,9 +615,9 @@ int cfb_infer_chunk_host(cfb_handle h, const void* h_in, int32_t in_dtype, int64
     CFB_CUDA(cudaEventRecord(h->ev[4], s));
     if (!no_staging && in_bytes >= ((size_t)64 << 20) && !is_pinned_host(h_in)) {
       if (!h->stager) h->stager = std::make_unique<HostStager>(h->p.device);
-      h->stager->upload(h_in, h->d_host_in, in_bytes, s);
+      h->stager->upload(h_in, d_in, in_bytes, s);
     } else {
-      CFB_CUDA(cudaMemcpyAsync(h->d_host_in, h_in, in_bytes, cudaMemcpyHostToDevice, s));
+      CFB_CUDA(cudaMemcpyAsync(d_in, h_in, in_bytes, cudaMemcpyHostToDevice, s));
     }
     CFB_CUDA(cudaEventRecord(h->ev[5], s));
     Progressive pg;
@@ -663,7 +629,7 @@ int cfb_infer_chunk_host(cfb_handle h, const void* h_in, int32_t in_dtype, int64
       pg.stager = h->stager.get();
     }
     const bool progressive = !h->p.has_myelin_threshold;
-    rc = infer_impl(h, h->d_host_in, in_dtype, cz, cy, cx, 0, 0, false, h->d_host_out, nullptr, s, progressive ? &pg : nullptr);
+    rc = infer_impl(h, d_in, in_dtype, cz, cy, cx, 0, 0, false, d_out, nullptr, s, progressive ? &pg : nullptr);
     if (rc != CFB_OK) {
       cudaStreamSynchronize(h->copy_stream);
       if (pg.stager) { try { pg.stager->drain(); } catch (...) {} }
@@ -671,8 +637,8 @@ int cfb_infer_chunk_host(cfb_handle h, const void* h_in, int32_t in_dtype, int64
     }
     CFB_CUDA(cudaEventRecord(h->ev[6], s));
     if (!progressive) {
-      if (pg.stager) pg.stager->push(h->d_host_out, h_out, out_bytes, s, h->copy_stream);
-      else CFB_CUDA(cudaMemcpyAsync(h_out, h->d_host_out, out_bytes, cudaMemcpyDeviceToHost, s));
+      if (pg.stager) pg.stager->push(d_out, h_out, out_bytes, s, h->copy_stream);
+      else CFB_CUDA(cudaMemcpyAsync(h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, s));
     }
     CFB_CUDA(cudaEventRecord(h->ev[7], s));
     CFB_CUDA(cudaStreamSynchronize(s));
@@ -690,21 +656,21 @@ int cfb_patch_forward_host(cfb_handle h, const float* h_patches, int32_t batch, 
     cudaStream_t s = h->own_stream;
     const int C = h->p.num_output_channels;
     const int64_t in_vol = vol(h->ip), out_vol = vol(h->op);
-    ensure(h->d_plugin_out, h->plugin_out_cap, (size_t)batch * C * out_vol * sizeof(float));
+    h->plugin_out.grow((size_t)batch * C * out_vol * sizeof(float));
     const int B = std::max(1, h->p.batch_size);
     for (int i = 0; i < batch; i += B) {
       const int nb = std::min(B, batch - i);
-      float* dst = h->d_plugin_out + (int64_t)i * C * out_vol;
+      float* dst = h->plugin_out.as<float>() + (int64_t)i * C * out_vol;
       if (h->p.framework == CFB_FRAMEWORK_IDENTITY) {
         float* stage = h->net.patch_input_buffer(nb);
         CFB_CUDA(cudaMemcpyAsync(stage, h_patches + (int64_t)i * in_vol, (size_t)nb * in_vol * sizeof(float), cudaMemcpyHostToDevice, s));
-        launch_crop_mask(stage, 1, h->ip, h->op, h->pcrop, h->d_mask, nb, dst, C, /*repeat=*/true, s);
+        launch_crop_mask(stage, 1, h->ip, h->op, h->pcrop, h->mask.as<float>(), nb, dst, C, /*repeat=*/true, s);
       } else {
         h->net.forward_from_host_patches(h_patches + (int64_t)i * in_vol, nb, s);
-        h->net.crop_mask(h->op, h->pcrop, h->d_mask, nb, dst, C, s);
+        h->net.crop_mask(h->op, h->pcrop, h->mask.as<float>(), nb, dst, C, s);
       }
     }
-    CFB_CUDA(cudaMemcpyAsync(h_out, h->d_plugin_out, (size_t)batch * C * out_vol * sizeof(float), cudaMemcpyDeviceToHost, s));
+    CFB_CUDA(cudaMemcpyAsync(h_out, h->plugin_out.as(), (size_t)batch * C * out_vol * sizeof(float), cudaMemcpyDeviceToHost, s));
     CFB_CUDA(cudaStreamSynchronize(s));
     return CFB_OK;
   });
@@ -730,13 +696,10 @@ int cfb_plugin_begin(cfb_handle h, const void* h_in, int32_t in_dtype, int64_t c
     cudaStream_t s = h->own_stream;
     prepare_chunk(h, cz, cy, cx, s);
     const size_t in_bytes = (size_t)cz * cy * cx * (in_dtype == CFB_DTYPE_U8 ? 1 : 4);
-    const size_t out_bytes = (size_t)h->p.num_output_channels * vol(h->out_size) * sizeof(float);
-    ensure(h->d_host_in, h->host_in_cap, in_bytes);
-    ensure(h->d_host_out, h->host_out_cap, out_bytes);
-    CFB_CUDA(cudaMemcpyAsync(h->d_host_in, h_in, in_bytes, cudaMemcpyHostToDevice, s));
-    CFB_CUDA(cudaMemsetAsync(h->d_flags, 0, 2 * sizeof(unsigned int), s));
-    launch_any_nonzero(h->d_host_in, in_dtype, cz * cy * cx, h->d_flags, s);
-    CFB_CUDA(cudaMemsetAsync(h->d_host_out, 0, out_bytes, s));
+    h->host_in.grow(in_bytes);
+    h->host_out.grow((size_t)h->p.num_output_channels * vol(h->geo.out) * sizeof(float));
+    CFB_CUDA(cudaMemcpyAsync(h->host_in.as(), h_in, in_bytes, cudaMemcpyHostToDevice, s));
+    start_chunk(h, h->host_in.as(), in_dtype, h->host_out.as<float>(), s);
     h->plugin_dtype = in_dtype;
     h->plugin_active = true;
     return CFB_OK;
@@ -750,9 +713,10 @@ int cfb_plugin_extract(cfb_handle h, int64_t first, int32_t nb, float* h_patches
     CFB_CUDA(cudaSetDevice(h->p.device));
     cudaStream_t s = h->own_stream;
     const size_t bytes = (size_t)nb * vol(h->ip) * sizeof(float);
-    ensure(h->d_plugin_in, h->plugin_in_cap, bytes);
-    launch_extract_patches(h->d_host_in, h->plugin_dtype, h->cached_chunk, h->d_patches + first, nb, h->ip, h->d_plugin_in, s);
-    CFB_CUDA(cudaMemcpyAsync(h_patches, h->d_plugin_in, bytes, cudaMemcpyDeviceToHost, s));
+    h->plugin_in.grow(bytes);
+    launch_extract_patches(h->host_in.as(), h->plugin_dtype, h->geo.size, h->patches.as<PatchPos>() + first, nb, h->ip,
+                           h->plugin_in.as<float>(), s);
+    CFB_CUDA(cudaMemcpyAsync(h_patches, h->plugin_in.as(), bytes, cudaMemcpyDeviceToHost, s));
     CFB_CUDA(cudaStreamSynchronize(s));
     return CFB_OK;
   });
@@ -766,11 +730,11 @@ int cfb_plugin_blend(cfb_handle h, int64_t first, int32_t nb, const float* h_mas
     cudaStream_t s = h->own_stream;
     const int C = h->p.num_output_channels;
     const size_t bytes = (size_t)nb * C * vol(h->op) * sizeof(float);
-    ensure(h->d_plugin_out, h->plugin_out_cap, bytes);
-    CFB_CUDA(cudaMemcpyAsync(h->d_plugin_out, h_masked_outputs, bytes, cudaMemcpyHostToDevice, s));
+    h->plugin_out.grow(bytes);
+    CFB_CUDA(cudaMemcpyAsync(h->plugin_out.as(), h_masked_outputs, bytes, cudaMemcpyHostToDevice, s));
     // already cropped and masked by the plugin: crop 0, no mask
-    launch_blend_patches(h->d_plugin_out, C, h->op, h->op, Int3{0, 0, 0}, nullptr, h->d_patches + first, nb,
-                         h->d_host_out, C, h->out_size, 1.0f, s);
+    launch_blend_patches(h->plugin_out.as<float>(), C, h->op, h->op, Int3{0, 0, 0}, nullptr, h->patches.as<PatchPos>() + first, nb,
+                         h->host_out.as<float>(), C, h->geo.out, 1.0f, s);
     CFB_CUDA(cudaStreamSynchronize(s));  // the caller may reuse its host buffer
     return CFB_OK;
   });
@@ -783,21 +747,14 @@ int cfb_plugin_end(cfb_handle h, float* h_out) {
     cudaStream_t s = h->own_stream;
     h->plugin_active = false;
     const int C = h->p.num_output_channels;
-    const int64_t nvox = vol(h->out_size);
-    const float* w = nullptr;
-    if (h->p.mask_output_chunk) { ensure_winv(h, s); w = h->d_winv; }
-    launch_normalize(h->d_host_out, w, true, C, nvox, h->d_flags + 1, h->d_flags, s);
-    if (h->p.has_myelin_threshold) launch_myelin_mask(h->d_host_out, C, nvox, h->p.mask_myelin_threshold, s);
-    unsigned int flags[2];
-    CFB_CUDA(cudaMemcpyAsync(flags, h->d_flags, sizeof(flags), cudaMemcpyDeviceToHost, s));
-    CFB_CUDA(cudaMemcpyAsync(h_out, h->d_host_out, (size_t)C * nvox * sizeof(float), cudaMemcpyDeviceToHost, s));
+    const int64_t nvox = vol(h->geo.out);
+    float* out = h->host_out.as<float>();
+    const float* w = h->p.mask_output_chunk ? inverse_weight(h, s) : nullptr;
+    finish_output(h, out, w, true, C, nvox, s);
+    CFB_CUDA(cudaMemcpyAsync(h_out, out, (size_t)C * nvox * sizeof(float), cudaMemcpyDeviceToHost, s));
+    const int rc = output_range_status(h, s);
     CFB_CUDA(cudaStreamSynchronize(s));
-    float vmax; std::memcpy(&vmax, &flags[1], 4);
-    if (h->p.check_output_range && !(vmax < 1.0001f)) {
-      set_last_error("output buffer should not be greater than 1 (max = " + std::to_string(vmax) + ")");
-      return CFB_ERR_OUTPUT_RANGE;
-    }
-    return CFB_OK;
+    return rc;
   });
 }
 

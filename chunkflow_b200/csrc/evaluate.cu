@@ -59,22 +59,6 @@ void ev_launch_pairs(const TS* seg, const void* gt, int32_t gt_dtype, int64_t n,
   CFB_LAUNCH_CHECK();
 }
 
-template <typename F>
-int guarded_eval(F&& f) {
-  try {
-    return f();
-  } catch (const std::invalid_argument& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_INVALID_ARGUMENT;
-  } catch (const CudaError& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_CUDA;
-  } catch (const std::exception& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_UNSUPPORTED;
-  }
-}
-
 }  // namespace
 }  // namespace cfb
 
@@ -87,7 +71,7 @@ extern "C" int64_t cfb_evaluate_workspace(int64_t table_slots) {
 
 extern "C" int cfb_contingency_device(const void* d_seg, int32_t seg_dtype, const void* d_gt, int32_t gt_dtype, int64_t z, int64_t y,
                                       int64_t x, void* d_workspace, int64_t table_slots, int64_t* num_pairs, void* stream) {
-  return guarded_eval([&]() -> int {
+  return guarded([&]() -> int {
     if (!d_seg || !d_gt || !d_workspace || !num_pairs) throw std::invalid_argument("evaluate: null argument");
     if (z <= 0 || y <= 0 || x <= 0 || z > INT32_MAX || y > INT32_MAX || x > INT32_MAX) throw std::invalid_argument("evaluate: bad volume size");
     const int64_t n = z * y * x;
@@ -121,7 +105,7 @@ extern "C" int cfb_contingency_device(const void* d_seg, int32_t seg_dtype, cons
 }
 
 extern "C" int cfb_contingency_scores(void* d_workspace, int64_t table_slots, double size_threshold, cfb_seg_scores* out, void* stream) {
-  return guarded_eval([&]() -> int {
+  return guarded([&]() -> int {
     if (!d_workspace || !out) throw std::invalid_argument("evaluate scores: null argument");
     if (out->struct_size != (int32_t)sizeof(cfb_seg_scores)) throw std::invalid_argument("evaluate scores: cfb_seg_scores size mismatch");
     ev_check_slots(table_slots);
@@ -157,7 +141,7 @@ extern "C" int cfb_contingency_scores(void* d_workspace, int64_t table_slots, do
 
 extern "C" int cfb_contingency_read(void* d_workspace, int64_t table_slots, int64_t num_pairs, uint64_t* h_seg, uint64_t* h_gt,
                                     uint32_t* h_count, void* stream) {
-  return guarded_eval([&]() -> int {
+  return guarded([&]() -> int {
     if (!d_workspace || num_pairs < 0 || num_pairs > table_slots) throw std::invalid_argument("evaluate read: bad argument");
     ev_check_slots(table_slots);
     if (num_pairs == 0) return CFB_OK;

@@ -341,14 +341,13 @@ void launch_crop_mask(const float* net, int cnet, Int3 ip, Int3 op, Int3 crop, c
   CFB_LAUNCH_CHECK();
 }
 
-void launch_weight_volume(const float* mask, Int3 op, const int* cover_z, const int* cover_y, const int* cover_x,
-                          const int* oz0, const int* oy0, const int* ox0, Int3 os, float* w, bool invert,
-                          cudaStream_t s, int z_begin, int z_end) {
+void launch_weight_volume(const float* mask, Int3 op, const CoverTables& t, Int3 os, float* w, bool invert, cudaStream_t s,
+                          int z_begin, int z_end) {
   if (z_end < 0) z_end = os.z;
   const int nz = z_end - z_begin;
   if (nz <= 0) return;
-  weight_volume_kernel<<<grid_for((int64_t)nz * os.y * os.x), kThreads, 0, s>>>(mask, op, cover_z, cover_y, cover_x, oz0, oy0, ox0,
-                                                                               os, w, invert, z_begin, nz);
+  weight_volume_kernel<<<grid_for((int64_t)nz * os.y * os.x), kThreads, 0, s>>>(mask, op, t.cover_z, t.cover_y, t.cover_x, t.ostart_z,
+                                                                               t.ostart_y, t.ostart_x, os, w, invert, z_begin, nz);
   CFB_LAUNCH_CHECK();
 }
 

@@ -29,11 +29,17 @@ void launch_identity_blend(const void* chunk, int in_dtype, Int3 chunk_size, Int
 void launch_crop_mask(const float* net, int cnet, Int3 in_patch, Int3 out_patch, Int3 crop, const float* mask,
                       int nb, float* out, int channels, bool repeat, cudaStream_t s);
 
+// Device tables of the weight-volume gather: per output axis, the cover table (kMaxCover patch axis-indices per
+// coordinate) and the output start of every patch axis-index.
+struct CoverTables {
+  const int *cover_z, *cover_y, *cover_x;
+  const int *ostart_z, *ostart_y, *ostart_x;
+};
+
 // a5 (reference inferencer.py:294-333): W(v) = sum over covering patches (in patch-list
 // order) of mask(v - o_p); writes 1/W if `invert`, else W.
-void launch_weight_volume(const float* mask, Int3 out_patch, const int* cover_z, const int* cover_y,
-                          const int* cover_x, const int* ostart_z, const int* ostart_y, const int* ostart_x,
-                          Int3 out_size, float* w, bool invert, cudaStream_t s, int z_begin = 0, int z_end = -1);
+void launch_weight_volume(const float* mask, Int3 out_patch, const CoverTables& t, Int3 out_size, float* w, bool invert,
+                          cudaStream_t s, int z_begin = 0, int z_end = -1);
 
 // dst[i] += src[i]: halo planes received from another rank (one chunk split over GPUs, BASELINE config #5).
 void launch_halo_add(float* dst, const float* src, int64_t n, cudaStream_t s);

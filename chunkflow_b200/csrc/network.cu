@@ -57,22 +57,17 @@ void Network::configure(int precision, Int3 patch, int batch) {
 }
 
 void Network::release() {
-  for (void* p : owned_) cudaFree(p);
-  owned_.clear();
+  for (DeviceBuffer& a : act_) a.reset();
   for (ConvLayer& L : layers_) { cudaFree(L.w); cudaFree(L.bias); free_packed(L.packed); }
   layers_.clear();
   for (cudaEvent_t e : prof_pool_) cudaEventDestroy(e);
   prof_pool_.clear();
   ready_ = false;
-  act_.fill(nullptr);
 }
 
 float* Network::patch_input_buffer(int nb) {
   if (nb > batch_) throw std::invalid_argument("batch larger than configured");
-  if (!act_[kIn]) {
-    CFB_CUDA(cudaMalloc(&act_[kIn], (size_t)vol(patch_) * batch_ * sizeof(float)));
-    owned_.push_back(act_[kIn]);
-  }
+  act_[kIn].grow((size_t)vol(patch_) * batch_ * sizeof(float));
   return f32(kIn);
 }
 
@@ -80,8 +75,7 @@ void Network::allocate() {
   if (act_[kOut]) return;
   patch_input_buffer(1);
   auto alloc = [&](Act a, size_t bytes_per_voxel, int level) {
-    CFB_CUDA(cudaMalloc(&act_[a], bytes_per_voxel * (size_t)(vol(patch_) >> (2 * level)) * batch_));
-    owned_.push_back(act_[a]);
+    act_[a].grow(bytes_per_voxel * (size_t)(vol(patch_) >> (2 * level)) * batch_);
   };
   alloc(kOut, sizeof(float) * std::max(cnet_, 1), 0);
   const size_t bytes = tensor_cores() ? sizeof(__half) * parts() : sizeof(float);  // per channel and voxel
@@ -269,21 +263,17 @@ void Network::copy_raw_output_to_host(float* h_out, cudaStream_t s) {
 
 int Network::debug_conv3(const float* h_in, int cin, Int3 size, const float* h_w, const float* h_b, int cout, bool relu,
                          float* h_out, cudaStream_t s) {
-  float *d_in = nullptr, *d_w = nullptr, *d_b = nullptr, *d_out = nullptr;
   const int64_t v = vol(size);
-  CFB_CUDA(cudaMalloc(&d_in, (size_t)cin * v * 4));
-  CFB_CUDA(cudaMalloc(&d_w, (size_t)cout * cin * 27 * 4));
-  CFB_CUDA(cudaMalloc(&d_b, (size_t)cout * 4));
-  CFB_CUDA(cudaMalloc(&d_out, (size_t)cout * v * 4));
+  DeviceBuffer in((size_t)cin * v * 4), w((size_t)cout * cin * 27 * 4), b((size_t)cout * 4), out((size_t)cout * v * 4);
+  float *d_in = in.as<float>(), *d_out = out.as<float>();
   CFB_CUDA(cudaMemcpyAsync(d_in, h_in, (size_t)cin * v * 4, cudaMemcpyHostToDevice, s));
-  CFB_CUDA(cudaMemcpyAsync(d_w, h_w, (size_t)cout * cin * 27 * 4, cudaMemcpyHostToDevice, s));
-  CFB_CUDA(cudaMemcpyAsync(d_b, h_b, (size_t)cout * 4, cudaMemcpyHostToDevice, s));
+  CFB_CUDA(cudaMemcpyAsync(w.as(), h_w, (size_t)cout * cin * 27 * 4, cudaMemcpyHostToDevice, s));
+  CFB_CUDA(cudaMemcpyAsync(b.as(), h_b, (size_t)cout * 4, cudaMemcpyHostToDevice, s));
   if (tensor_cores()) {
-    if (cin % 16) { cudaFree(d_in); cudaFree(d_w); cudaFree(d_b); cudaFree(d_out); throw std::runtime_error("the wgmma convolution needs cin % 16 == 0"); }
+    if (cin % 16) throw std::runtime_error("the wgmma convolution needs cin % 16 == 0");
     const int P = parts();
-    __half *c_in = nullptr, *c_out = nullptr;
-    CFB_CUDA(cudaMalloc(&c_in, (size_t)cin * P * v * 2));
-    CFB_CUDA(cudaMalloc(&c_out, (size_t)cout * P * v * 2));
+    DeviceBuffer cp8_in((size_t)cin * P * v * 2), cp8_out((size_t)cout * P * v * 2);
+    __half *c_in = cp8_in.as<__half>(), *c_out = cp8_out.as<__half>();
     PackedConv pk;
     pack_conv3_weights(h_w, h_b, cin, cout, fmt(), pk);
     launch_planar_to_cp8(d_in, c_in, cin, fmt(), 1, size, s);
@@ -293,15 +283,13 @@ int Network::debug_conv3(const float* h_in, int cin, Int3 size, const float* h_w
     launch_cp8_to_planar(c_out, d_out, cout, fmt(), 1, size, s);
     CFB_CUDA(cudaMemcpyAsync(h_out, d_out, (size_t)cout * v * 4, cudaMemcpyDeviceToHost, s));
     cudaError_t err = cudaStreamSynchronize(s);
-    cudaFree(c_in); cudaFree(c_out); free_packed(pk);
-    cudaFree(d_in); cudaFree(d_w); cudaFree(d_b); cudaFree(d_out);
+    free_packed(pk);
     CFB_CUDA(err);
     return CFB_OK;
   }
-  launch_conv3_f32(d_in, cin, nullptr, 0, d_w, d_b, d_out, cout, 1, size, relu, s);
+  launch_conv3_f32(d_in, cin, nullptr, 0, w.as<float>(), b.as<float>(), d_out, cout, 1, size, relu, s);
   CFB_CUDA(cudaMemcpyAsync(h_out, d_out, (size_t)cout * v * 4, cudaMemcpyDeviceToHost, s));
   CFB_CUDA(cudaStreamSynchronize(s));
-  cudaFree(d_in); cudaFree(d_w); cudaFree(d_b); cudaFree(d_out);
   return CFB_OK;
 }
 

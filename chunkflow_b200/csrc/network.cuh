@@ -75,8 +75,8 @@ class Network {
     return precision_ == CFB_PRECISION_F16X3_UMMA ? kFmtF16x2 : precision_ == CFB_PRECISION_F16F8_UMMA ? kFmtF16F8 : kFmtF16;
   }
   int parts() const { return fmt_planes(fmt()); }
-  float* f32(Act a) const { return static_cast<float*>(act_[a]); }
-  __half* cp8(Act a) const { return static_cast<__half*>(act_[a]); }
+  float* f32(Act a) const { return act_[a].as<float>(); }
+  __half* cp8(Act a) const { return act_[a].as<__half>(); }
 
   struct Span { int id; cudaEvent_t a, b; };
   void prof_begin(const char* name, cudaStream_t s);
@@ -96,9 +96,8 @@ class Network {
   int cnet_ = 0;
   FirstConvW first_w_{};              // host copy of the first layer, passed to its kernel by value
   std::vector<ConvLayer> layers_;     // by index into the layer table
-  std::vector<void*> owned_;
   // (batch, C, Z, Y, X) fp32 for kIn, kOut and every activation of the simt mode, CP8 for the tensor-core modes
-  std::array<void*, kNumActs> act_{};
+  std::array<DeviceBuffer, kNumActs> act_;
 };
 
 }  // namespace cfb

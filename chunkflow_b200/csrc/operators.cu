@@ -28,22 +28,6 @@ int sm_count_ops() {
   return n;
 }
 
-template <typename F>
-int guarded_op(F&& f) {
-  try {
-    return f();
-  } catch (const std::invalid_argument& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_INVALID_ARGUMENT;
-  } catch (const CudaError& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_CUDA;
-  } catch (const std::exception& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_UNSUPPORTED;
-  }
-}
-
 // ------------------------------------------------------------------------------------------
 // normalize-contrast
 // ------------------------------------------------------------------------------------------
@@ -412,7 +396,7 @@ extern "C" {
 int cfb_normalize_contrast_device(void* d_image, int64_t z, int64_t y, int64_t x, double lower_clip_fraction,
                                   double upper_clip_fraction, int32_t minval, int32_t maxval, int32_t per_section,
                                   void* stream) {
-  return guarded_op([&]() -> int {
+  return guarded([&]() -> int {
     check_dims(1, z, y, x);
     if (!d_image) throw std::invalid_argument("normalize_contrast: null image");
     if (minval < 0 || maxval > 255 || minval > maxval) throw std::invalid_argument("normalize_contrast: need 0 <= minval <= maxval <= 255");
@@ -450,7 +434,7 @@ int cfb_normalize_contrast_device(void* d_image, int64_t z, int64_t y, int64_t x
 
 int cfb_maskout_device(void* d_chunk, int32_t chunk_dtype, int64_t channels, int64_t z, int64_t y, int64_t x,
                        const void* d_mask, int32_t mask_dtype, int64_t fz, int64_t fy, int64_t fx, void* stream) {
-  return guarded_op([&]() -> int {
+  return guarded([&]() -> int {
     check_dims(channels, z, y, x);
     if (!d_chunk || !d_mask) throw std::invalid_argument("maskout: null pointer");
     if (fz < 1 || fy < 1 || fx < 1 || z % fz || y % fy || x % fx)
@@ -479,7 +463,7 @@ int cfb_maskout_device(void* d_chunk, int32_t chunk_dtype, int64_t channels, int
 
 int cfb_crop_margin_device(const void* d_src, int32_t dtype, int64_t channels, int64_t z, int64_t y, int64_t x,
                            const int64_t margin[6], void* d_dst, void* stream) {
-  return guarded_op([&]() -> int {
+  return guarded([&]() -> int {
     check_dims(channels, z, y, x);
     if (!d_src || !d_dst || !margin) throw std::invalid_argument("crop_margin: null pointer");
     for (int i = 0; i < 6; ++i)
@@ -506,7 +490,7 @@ int cfb_crop_margin_device(const void* d_src, int32_t dtype, int64_t channels, i
 
 int cfb_quantize_device(const float* d_affinity, int64_t channels, int64_t z, int64_t y, int64_t x, int32_t mode,
                         uint8_t* d_out, void* stream) {
-  return guarded_op([&]() -> int {
+  return guarded([&]() -> int {
     check_dims(channels, z, y, x);
     if (!d_affinity || !d_out) throw std::invalid_argument("quantize: null pointer");
     const int64_t n = z * y * x;

@@ -57,22 +57,6 @@ LtTable lt_table(void* d_workspace, int64_t slots) {
   return t;
 }
 
-template <typename F>
-int guarded_relabel(F&& f) {
-  try {
-    return f();
-  } catch (const std::invalid_argument& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_INVALID_ARGUMENT;
-  } catch (const CudaError& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_CUDA;
-  } catch (const std::exception& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_UNSUPPORTED;
-  }
-}
-
 template <typename TI>
 void lt_launch_apply(const TI* in, int64_t n, const LtTable& t, void* out, int32_t out_dtype, cudaStream_t s) {
   const int grid = lt_grid(ceil_div64(n, 16 / (int64_t)sizeof(TI)));
@@ -94,7 +78,7 @@ extern "C" int64_t cfb_label_table_workspace(int64_t voxels, int64_t table_slots
 
 extern "C" int cfb_label_table_device(const void* d_labels, int32_t dtype, int64_t z, int64_t y, int64_t x, void* d_workspace,
                                       int64_t table_slots, int64_t* num_labels, void* stream) {
-  return guarded_relabel([&]() -> int {
+  return guarded([&]() -> int {
     if (!d_labels || !d_workspace || !num_labels) throw std::invalid_argument("label table: null argument");
     if (z <= 0 || y <= 0 || x <= 0 || z > INT32_MAX || y > INT32_MAX || x > INT32_MAX) throw std::invalid_argument("label table: bad volume size");
     const int64_t n = z * y * x;
@@ -125,7 +109,7 @@ extern "C" int cfb_label_table_device(const void* d_labels, int32_t dtype, int64
 
 extern "C" int cfb_label_table_read(void* d_workspace, int64_t table_slots, int64_t num_labels, uint64_t* h_ids, uint32_t* h_counts,
                                     uint32_t* h_first, void* stream) {
-  return guarded_relabel([&]() -> int {
+  return guarded([&]() -> int {
     if (!d_workspace || num_labels < 0 || num_labels > table_slots) throw std::invalid_argument("label table read: bad argument");
     lt_check_slots(table_slots);
     if (num_labels == 0) return CFB_OK;
@@ -156,7 +140,7 @@ extern "C" int cfb_label_table_read(void* d_workspace, int64_t table_slots, int6
 extern "C" int cfb_label_table_plan(void* d_workspace, int64_t table_slots, int64_t voxels, int32_t use_dust, int64_t dust_threshold,
                                     const uint64_t* d_keep_ids, int64_t num_keep, int32_t renumber, uint64_t base_id,
                                     int64_t* num_dust, int64_t* num_survivors, uint64_t* new_max, void* stream) {
-  return guarded_relabel([&]() -> int {
+  return guarded([&]() -> int {
     if (!d_workspace) throw std::invalid_argument("label plan: null workspace");
     lt_check_voxels(voxels);
     lt_check_slots(table_slots);
@@ -212,7 +196,7 @@ extern "C" int cfb_label_table_plan(void* d_workspace, int64_t table_slots, int6
 
 extern "C" int cfb_label_apply_device(const void* d_in, int32_t in_dtype, int64_t voxels, void* d_workspace, int64_t table_slots,
                                       void* d_out, int32_t out_dtype, void* stream) {
-  return guarded_relabel([&]() -> int {
+  return guarded([&]() -> int {
     if (!d_in || !d_workspace || !d_out) throw std::invalid_argument("label apply: null argument");
     lt_check_voxels(voxels);
     lt_check_slots(table_slots);

@@ -136,22 +136,6 @@ WsGeom ws_geom(int64_t z, int64_t y, int64_t x) {
   return g;
 }
 
-template <typename F>
-int guarded_seg(F&& f) {
-  try {
-    return f();
-  } catch (const std::invalid_argument& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_INVALID_ARGUMENT;
-  } catch (const CudaError& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_CUDA;
-  } catch (const std::exception& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_UNSUPPORTED;
-  }
-}
-
 int grid_for(int64_t items) {
   int64_t b = ceil_div64(items, kT);
   return (int)std::max<int64_t>(1, std::min<int64_t>(b, 132 * 16));
@@ -165,7 +149,7 @@ using namespace cfb;
 extern "C" int cfb_connected_components_device(const void* d_in, int32_t in_dtype, int64_t z, int64_t y, int64_t x, float threshold,
                                                int32_t connectivity, uint32_t* d_labels, void* d_workspace, uint32_t* num_labels,
                                                void* stream) {
-  try {
+  return guarded([&]() -> int {
     if (!d_in || !d_labels || !d_workspace) throw std::invalid_argument("null argument");
     if (z <= 0 || y <= 0 || x <= 0 || z > INT32_MAX || y > INT32_MAX || x > INT32_MAX) throw std::invalid_argument("bad volume size");
     const int64_t n = z * y * x;
@@ -202,16 +186,7 @@ extern "C" int cfb_connected_components_device(const void* d_in, int32_t in_dtyp
       CFB_CUDA(cudaStreamSynchronize(s));
     }
     return CFB_OK;
-  } catch (const std::invalid_argument& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_INVALID_ARGUMENT;
-  } catch (const CudaError& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_CUDA;
-  } catch (const std::exception& ex) {
-    set_last_error(ex.what());
-    return CFB_ERR_UNSUPPORTED;
-  }
+  });
 }
 
 extern "C" int64_t cfb_connected_components_workspace(int64_t z, int64_t y, int64_t x) {
@@ -230,7 +205,7 @@ extern "C" int64_t cfb_watershed_workspace(int64_t z, int64_t y, int64_t x) {
 extern "C" int cfb_watershed_device(const float* d_affs, int32_t flip_channel, int64_t z, int64_t y, int64_t x, float aff_threshold_low,
                                     float aff_threshold_high, uint32_t* d_fragments, void* d_workspace, uint32_t* num_fragments,
                                     void* stream) {
-  return guarded_seg([&]() -> int {
+  return guarded([&]() -> int {
     if (!d_affs || !d_fragments || !d_workspace) throw std::invalid_argument("watershed: null argument");
     if (!(aff_threshold_low < aff_threshold_high)) throw std::invalid_argument("watershed: need aff_threshold_low < aff_threshold_high");
     const WsGeom g = ws_geom(z, y, x);
@@ -291,7 +266,7 @@ extern "C" int64_t cfb_region_graph_workspace(int64_t table_slots) {
 
 extern "C" int cfb_region_graph_device(const float* d_affs, int32_t flip_channel, const uint32_t* d_fragments, int64_t z, int64_t y,
                                        int64_t x, void* d_workspace, int64_t table_slots, int64_t* num_edges, void* stream) {
-  return guarded_seg([&]() -> int {
+  return guarded([&]() -> int {
     if (!d_affs || !d_fragments || !d_workspace || !num_edges) throw std::invalid_argument("region graph: null argument");
     if (table_slots < 2 || (table_slots & (table_slots - 1)) || table_slots >= ((int64_t)1 << 31))
       throw std::invalid_argument("region graph: table_slots must be a power of two below 2^31");
@@ -321,7 +296,7 @@ extern "C" int cfb_region_graph_device(const float* d_affs, int32_t flip_channel
 
 extern "C" int cfb_region_graph_read(void* d_workspace, int64_t table_slots, int64_t num_edges, uint32_t* h_u, uint32_t* h_v,
                                      uint64_t* h_sum_fixed, uint32_t* h_count, void* stream) {
-  return guarded_seg([&]() -> int {
+  return guarded([&]() -> int {
     if (!d_workspace || table_slots < 2 || num_edges < 0 || num_edges > table_slots) throw std::invalid_argument("region graph read: bad argument");
     if (num_edges == 0) return CFB_OK;
     if (!h_u || !h_v || !h_sum_fixed || !h_count) throw std::invalid_argument("region graph read: null output");
@@ -360,7 +335,7 @@ extern "C" int cfb_region_graph_read(void* d_workspace, int64_t table_slots, int
 
 extern "C" int cfb_relabel_device(const uint32_t* d_labels, int64_t n, const uint32_t* d_map, int64_t map_size, uint32_t* d_out,
                                   void* stream) {
-  return guarded_seg([&]() -> int {
+  return guarded([&]() -> int {
     if (!d_labels || !d_map || !d_out || n < 0 || map_size < 0 || map_size > (int64_t)UINT32_MAX) throw std::invalid_argument("relabel: bad argument");
     if (n == 0) return CFB_OK;
     relabel_map_kernel<<<grid_for(n), kT, 0, (cudaStream_t)stream>>>(d_labels, n, d_map, (uint32_t)map_size, d_out);

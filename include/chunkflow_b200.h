@@ -125,6 +125,9 @@ int cfb_make_patch_mask(const int32_t patch_size[3], const int32_t overlap[3], f
 /* Copies the fp32 patch mask (prod(output_patch_size) floats) to host memory. */
 int cfb_patch_mask(cfb_handle h, float* host_out);
 
+/* Every call that takes a chunk shape (cz, cy, cx) returns CFB_ERR_INVALID_ARGUMENT for a chunk smaller than the
+ * input patch, a dimension above INT32_MAX, or an output crop margin that leaves no output voxel. */
+
 /* Patch grid for a chunk of the given size: writes the number of patches and, if
  * starts_zyx != NULL, up to `capacity` chunk-local input start triples (z,y,x per patch,
  * z-major then y then x, last patch per axis clamped). */
