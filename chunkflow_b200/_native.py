@@ -16,7 +16,7 @@ OK = 0
 ERR_INVALID_ARGUMENT, ERR_CUDA, ERR_WEIGHTS, ERR_OUTPUT_RANGE, ERR_UNSUPPORTED, ERR_CAPACITY = -1, -2, -3, -4, -5, -6
 FRAMEWORK_UNET3L, FRAMEWORK_IDENTITY = 0, 1
 PRECISION_F32_SIMT, PRECISION_F16X3_UMMA, PRECISION_F16_UMMA, PRECISION_F16F8_UMMA = 0, 1, 2, 3
-DTYPE_U8, DTYPE_F32, DTYPE_U32, DTYPE_U64 = 0, 1, 2, 3
+DTYPE_U8, DTYPE_F32, DTYPE_U32, DTYPE_U64, DTYPE_BOOL = 0, 1, 2, 3, 4
 AUGMENT_NONE, AUGMENT_REFERENCE, AUGMENT_SPATIAL = 0, 1, 2
 QUANTIZE_XY, QUANTIZE_Z = 0, 1
 
@@ -34,7 +34,7 @@ EXPORTS = (
     "cfb_region_graph_read", "cfb_agglomerate_edges_host", "cfb_relabel_device",
     "cfb_evaluate_workspace", "cfb_contingency_device", "cfb_contingency_scores", "cfb_contingency_read",
     "cfb_label_table_workspace", "cfb_label_table_device", "cfb_label_table_read", "cfb_label_table_plan",
-    "cfb_label_apply_device",
+    "cfb_label_apply_device", "cfb_downsample_average_device", "cfb_downsample_workspace", "cfb_downsample_segmentation_device",
 )
 
 
@@ -157,6 +157,9 @@ def load() -> C.CDLL:
     lib.cfb_label_table_plan.argtypes = [vp, i64, i64, i32, i64, vp, i64, i32, C.c_uint64, C.POINTER(i64), C.POINTER(i64),
                                          C.POINTER(C.c_uint64), vp]
     lib.cfb_label_apply_device.argtypes = [vp, i32, i64, vp, i64, vp, i32, vp]
+    lib.cfb_downsample_average_device.argtypes = [vp, i64, i64, i64, C.POINTER(i64 * 3), vp, vp]
+    lib.cfb_downsample_workspace.argtypes = [i32, i64, i64, i64, C.POINTER(i64 * 3), C.POINTER(i64 * 3), C.POINTER(i64)]
+    lib.cfb_downsample_segmentation_device.argtypes = [vp, i32, i64, i64, i64, C.POINTER(i64 * 3), vp, vp, vp]
     for name in EXPORTS:
         getattr(lib, name)   # every declared symbol must be there
     _lib = lib
@@ -397,6 +400,53 @@ def label_apply_device(d_in: int, in_dtype: int, voxels: int, d_workspace: int, 
         raise ValueError("voxels must be in [1, 2^32 - 2]")
     check(load().cfb_label_apply_device(C.c_void_p(d_in), in_dtype, int(voxels), C.c_void_p(d_workspace), slots, C.c_void_p(d_out),
                                         out_dtype, C.c_void_p(stream)))
+
+
+# ---- `downsample` (include/chunkflow_b200.h, DESIGN.md section 0, row f7) ----
+SEGMENTATION_DOWNSAMPLE_DTYPES = (DTYPE_U32, DTYPE_U64, DTYPE_BOOL)
+
+
+def _zyx_and_factor(zyx, factor):
+    zyx, factor = tuple(int(v) for v in zyx), tuple(int(v) for v in factor)
+    if len(zyx) != 3 or min(zyx) <= 0:
+        raise ValueError(f"a volume is (z, y, x) with positive sizes, not {zyx}")
+    if len(factor) != 3:
+        raise ValueError(f"the factor is (z, y, x), not {factor}")
+    if min(factor) <= 0:
+        raise ValueError(f"Factors less than one don't make sense. Factor: {factor}")
+    return zyx, (C.c_int64 * 3)(*factor)
+
+
+def _check_refusal(code: int) -> None:
+    """A refused factor (the reference raises on it) is a ValueError, like the reference's own refusals."""
+    if code == ERR_INVALID_ARGUMENT:
+        raise ValueError(load().cfb_last_error().decode("utf-8", "replace"))
+    check(code)
+
+
+def downsample_average_device(d_in: int, zyx, factor, d_out: int, stream: int = 0) -> None:
+    """uint8 averaging of the (z, y, x) volume at ``d_in`` into ceil(zyx / factor) voxels at ``d_out``."""
+    zyx, f = _zyx_and_factor(zyx, factor)
+    _check_refusal(load().cfb_downsample_average_device(C.c_void_p(d_in), *zyx, C.byref(f), C.c_void_p(d_out), C.c_void_p(stream)))
+
+
+def downsample_workspace(dtype: int, zyx, factor) -> tuple:
+    """The plan of a segmentation factor (no device needed) -> (output (z, y, x), workspace bytes); ValueError when refused."""
+    if dtype not in SEGMENTATION_DOWNSAMPLE_DTYPES:
+        raise TypeError("a segmentation to downsample is DTYPE_U32, DTYPE_U64 or DTYPE_BOOL")
+    zyx, f = _zyx_and_factor(zyx, factor)
+    out, work = (C.c_int64 * 3)(), C.c_int64()
+    _check_refusal(load().cfb_downsample_workspace(int(dtype), *zyx, C.byref(f), C.byref(out), C.byref(work)))
+    return tuple(out), int(work.value)
+
+
+def downsample_segmentation_device(d_in: int, dtype: int, zyx, factor, d_workspace: int, d_out: int, stream: int = 0) -> None:
+    """Mode pooling (countless) or striding of the (z, y, x) segmentation at ``d_in``, level after level, into ``d_out``."""
+    if dtype not in SEGMENTATION_DOWNSAMPLE_DTYPES:
+        raise TypeError("a segmentation to downsample is DTYPE_U32, DTYPE_U64 or DTYPE_BOOL")
+    zyx, f = _zyx_and_factor(zyx, factor)
+    _check_refusal(load().cfb_downsample_segmentation_device(C.c_void_p(d_in), int(dtype), *zyx, C.byref(f),
+                                                             C.c_void_p(d_workspace or None), C.c_void_p(d_out), C.c_void_p(stream)))
 
 
 def device_memory(device: int = 0) -> tuple:

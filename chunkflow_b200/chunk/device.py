@@ -490,5 +490,41 @@ class DeviceChunk:
         the next chunk -- 0 for an all-zero chunk whatever ``base_id``: the reference's value, kept."""
         return self._relabel(renumber=True, base_id=base_id, table_slots=table_slots)[3]
 
+    # ---- `downsample`: uint8 averaging, countless mode pooling of segmentations ---------------------------------
+    def downsample(self, factor=(2, 2, 2)) -> "DeviceChunk":
+        """The reference's `downsample` command (flow/flow.py:1545-1573) on the device: a (z,y,x) uint8 image is averaged, a
+        (z,y,x) int32 / uint32 / int64 / uint64 / bool segmentation is mode-pooled (countless) or strided level after level
+        (csrc/downsample.cu; the arithmetic of the reference's vendored lib/igneous/downsample.py, see
+        include/chunkflow_b200.h for the rules, the quirks kept and the refusals).  int32 holds uint32 ids and int64 the
+        uint64 bit pattern.  Returns a new chunk with ``voxel_offset // factor``, ``voxel_size * factor`` and the same
+        ``layer_type``; the input is not changed.  A refused factor raises ValueError before any kernel runs."""
+        torch = _torch()
+        f = tuple(int(v) for v in factor)
+        if len(f) != 3:
+            raise ValueError(f"the factor is (z, y, x), not {factor}")
+        t = self.tensor
+        codes = {torch.int32: _native.DTYPE_U32, torch.int64: _native.DTYPE_U64, torch.bool: _native.DTYPE_BOOL}
+        for name, code in (("uint32", _native.DTYPE_U32), ("uint64", _native.DTYPE_U64)):
+            if hasattr(torch, name):
+                codes[getattr(torch, name)] = code
+        if t.ndim != 3 or (t.dtype != torch.uint8 and t.dtype not in codes):
+            raise TypeError(f'only support image or segmentation, but got: {t.dtype}')
+        with self._on_device():
+            if t.dtype == torch.uint8:
+                shape = tuple(-(-s // k) for s, k in zip(t.shape, f)) if min(f) > 0 else None
+                out = torch.empty(shape or (0,), dtype=torch.uint8, device=t.device)
+                _native.downsample_average_device(t.data_ptr(), t.shape, f, out.data_ptr(), self._stream())
+            else:
+                code = codes[t.dtype]
+                shape, work_bytes = _native.downsample_workspace(code, t.shape, f)
+                out = torch.empty(shape, dtype=t.dtype, device=t.device)
+                work = torch.empty(work_bytes, dtype=torch.uint8, device=t.device) if work_bytes else None
+                _native.downsample_segmentation_device(t.data_ptr(), code, t.shape, f, work.data_ptr() if work is not None else 0,
+                                                       out.data_ptr(), self._stream())
+                del work   # the caching allocator keeps it for the stream until the levels have run
+        fc = Cartesian(*f)
+        return DeviceChunk(out, voxel_offset=self.voxel_offset // fc,
+                           voxel_size=None if self.voxel_size is None else self.voxel_size * fc, layer_type=self.layer_type)
+
     def __repr__(self):
         return f"DeviceChunk(shape={self.shape}, dtype={self.dtype}, voxel_offset={tuple(self.voxel_offset)}, device={self.tensor.device})"

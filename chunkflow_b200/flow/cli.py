@@ -301,6 +301,28 @@ def agglomerate(tasks, name, input_chunk_name, output_chunk_name, threshold, aff
         yield task
 
 
+@main.command("downsample")
+@click.option("--input-chunk-name", "-i", type=str, default="chunk", help="input chunk name")
+@click.option("--output-chunk-name", "-o", type=str, default="chunk", help="output chunk name")
+@click.option("--factor", "-f", type=click.INT, nargs=3, default=(2, 2, 2), help="downsample factor in zyx. The default is 2x2x2.")
+@operator
+def downsample(tasks, input_chunk_name, output_chunk_name, factor):
+    """Downsample a chunk (reference flow/flow.py:1545-1573): a uint8 image is averaged, an integer or boolean segmentation
+    mode-pooled.  A pyramid is a chain (`downsample -o mip1 downsample -i mip1 -o mip2`), a thumbnail
+    `quantize --mode z downsample -f 1 2 2 ...`.  A host chunk comes back to the host, a GPU-resident one stays there."""
+    import torch
+    for task in tasks:
+        if task is not None:
+            dev, was_host = _on_device(task[input_chunk_name], "cuda:0")
+            out = dev.downsample(factor)
+            torch.cuda.synchronize(out.tensor.device)
+            if was_host:
+                out = Chunk(out.to_chunk().array, voxel_offset=out.voxel_offset, voxel_size=out.voxel_size,
+                            layer_type=getattr(task[input_chunk_name], "_layer_type", None))
+            task[output_chunk_name] = out
+        yield task
+
+
 @main.command("evaluate-segmentation")
 @click.option("--segmentation-chunk-name", "-s", type=str, default="chunk", help="chunk name of segmentation")
 @click.option("--groundtruth-chunk-name", "-g", type=str, default="groundtruth")

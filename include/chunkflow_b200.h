@@ -26,6 +26,7 @@
  *                                 Segmentation.evaluate   chunk/segmentation.py:33-67 (-> lib/gala/evaluate.py)
  *   cfb_label_table_*, cfb_label_apply_device
  *                                 Segmentation.remap / mask_fragments / mask_except   chunk/segmentation.py:69-109
+ *   cfb_downsample_*              the `downsample` command   flow/flow.py:1545-1573 (-> lib/igneous/downsample.py)
  *
  * Plain pointers and sizes only -- no torch types.  Device pointers are raw CUDA device
  * addresses (e.g. torch.Tensor.data_ptr()) owned by the caller.  All functions return
@@ -78,6 +79,7 @@ extern "C" {
 #define CFB_DTYPE_F32 1
 #define CFB_DTYPE_U32 2 /* connected components on an integer segmentation */
 #define CFB_DTYPE_U64 3 /* segmentation evaluation and clean-up: 64-bit label ids */
+#define CFB_DTYPE_BOOL 4 /* downsample: a boolean segmentation (one byte per voxel), always strided */
 
 typedef struct cfb_engine* cfb_handle;
 
@@ -387,6 +389,48 @@ int cfb_label_table_plan(void* d_workspace, int64_t table_slots, int64_t voxels,
                          int64_t* num_survivors, uint64_t* new_max, void* stream);
 int cfb_label_apply_device(const void* d_in, int32_t in_dtype, int64_t voxels, void* d_workspace, int64_t table_slots,
                            void* d_out, int32_t out_dtype, void* stream);
+
+/* `downsample` (DESIGN.md section 0, row f7): the reference's command (flow/flow.py:1545-1573) averages a uint8 image and
+ * mode-pools an integer or boolean segmentation by a factor (fz, fy, fx) of the (z,y,x) C-order volume.  It calls tinybrain,
+ * a third-party package outside the reference tree (parity unpinned); the arithmetic pinned here, bit for bit, is the
+ * reference's vendored numpy downsampler (lib/igneous/downsample.py), restated in oracle/downsample_oracle.py.  The output
+ * of every level is ceil(extent / factor) per axis, except where a 2x2 step rounds an odd side up (below).
+ *
+ * cfb_downsample_average_device  downsample_with_averaging (:103-125): out = floor(block sum / voxels in the block), the
+ *     blocks at the far edges clipped to the voxels that exist; that is the reference's float32 sum, float64 division and
+ *     cast, for blocks of at most 65793 voxels (65793 * 255 < 2^24).  Larger blocks and factors below one return
+ *     CFB_ERR_INVALID_ARGUMENT.  (1,1,1) copies the input.
+ * cfb_downsample_segmentation_device  downsample_segmentation (:154-253), one level after the other from the element kind,
+ *     the level's shape and the remaining factor f:
+ *       all f == 1                                    done (no level: the input is copied);
+ *       CFB_DTYPE_BOOL, or prod(f) not a power of two stride  out = in[::fz, ::fy, ::fx]  (:429-441), the last level;
+ *       no f == 1, every extent even                  countless3d (:326-400), then f // 2;
+ *       some f == 1                                   countless2d (:256-295) on the other two axes, the first axis with
+ *                                                     f == 1 preserved, then f // 2 with the preserved axis kept at 1;
+ *       otherwise (an odd extent)                     stride.
+ *     countless2d: an odd side first gets a copy of its first row in front (odd_to_even2d :54-92), so output j reads inputs
+ *     (max(2j - 1, 0), 2j); with a, b, c, d the pair's (lo,lo), (lo,hi), (hi,lo), (hi,hi) voxels: a if a == b or a == c, else
+ *     b if b == c, else d.  countless3d, the 8 voxels in (z,y,x) ndindex order: the first value seen >= 4 times, else >= 3
+ *     times, else >= 2 times among the first 7 voxels, else the 8th voxel.
+ *     Kept quirks: the reference offsets ids by +1 in the stored width and takes 0 as "no pick", so the all-ones id
+ *     (2^32 - 1, 2^64 - 1) never counts as a pick in countless3d, nor in countless2d for CFB_DTYPE_U64 (it widens 32-bit
+ *     ids first).  A 2x2 step halves both other axes even when one of them has f == 1 -- its f // 2 is then 0, which the
+ *     reference refuses, and so is the factor here.
+ *     Deviations: the reference recurses with factor / 2, a float, and raises on every second level; here f // 2 is used,
+ *     so that higher powers of two (4,4,4), (1,4,4), ... run level after level as its documentation intends.  The 2x2 step
+ *     also takes the 3-D arrays on which the reference's raises.
+ *     Refused with CFB_ERR_INVALID_ARGUMENT before any kernel: a factor below one, a product above 2^31 - 1, and every
+ *     factor whose recursion reaches a factor of 0 ((1,1,2), (1,2,4), (2,2,4) on even shapes, ...).
+ * cfb_downsample_workspace  the plan of a segmentation factor without a device: the output shape and the bytes of device
+ *     memory the intermediate levels need (0 for one level); CFB_ERR_INVALID_ARGUMENT when the factor is refused.
+ * dtype: CFB_DTYPE_U32 (also int32 volumes holding uint32 ids), CFB_DTYPE_U64 (also the bit pattern of int64 volumes) or
+ * CFB_DTYPE_BOOL.  The input is only read; it may start at any address; input, output and workspace must not overlap. */
+int cfb_downsample_average_device(const uint8_t* d_in, int64_t z, int64_t y, int64_t x, const int64_t factor[3], uint8_t* d_out,
+                                  void* stream);
+int cfb_downsample_workspace(int32_t dtype, int64_t z, int64_t y, int64_t x, const int64_t factor[3], int64_t out_zyx[3],
+                             int64_t* workspace_bytes);
+int cfb_downsample_segmentation_device(const void* d_in, int32_t dtype, int64_t z, int64_t y, int64_t x, const int64_t factor[3],
+                                       void* d_workspace, void* d_out, void* stream);
 
 #ifdef __cplusplus
 }
