@@ -35,6 +35,7 @@ EXPORTS = (
     "cfb_evaluate_workspace", "cfb_contingency_device", "cfb_contingency_scores", "cfb_contingency_read",
     "cfb_label_table_workspace", "cfb_label_table_device", "cfb_label_table_read", "cfb_label_table_plan",
     "cfb_label_apply_device", "cfb_downsample_average_device", "cfb_downsample_workspace", "cfb_downsample_segmentation_device",
+    "cfb_gaussian_filter_workspace", "cfb_gaussian_filter_device", "cfb_median_filter_device",
 )
 
 
@@ -160,6 +161,10 @@ def load() -> C.CDLL:
     lib.cfb_downsample_average_device.argtypes = [vp, i64, i64, i64, C.POINTER(i64 * 3), vp, vp]
     lib.cfb_downsample_workspace.argtypes = [i32, i64, i64, i64, C.POINTER(i64 * 3), C.POINTER(i64 * 3), C.POINTER(i64)]
     lib.cfb_downsample_segmentation_device.argtypes = [vp, i32, i64, i64, i64, C.POINTER(i64 * 3), vp, vp, vp]
+    dp = C.POINTER(C.c_double)
+    lib.cfb_gaussian_filter_workspace.argtypes = [i32, i64, i64, i64, i64, C.POINTER(i64)]
+    lib.cfb_gaussian_filter_device.argtypes = [vp, i32, i64, i64, i64, i64, dp, i32, dp, i32, dp, i32, vp, i64, vp]
+    lib.cfb_median_filter_device.argtypes = [vp, i32, i64, i64, i64, i64, C.POINTER(i64 * 4), i32, vp, vp]
     for name in EXPORTS:
         getattr(lib, name)   # every declared symbol must be there
     _lib = lib
@@ -447,6 +452,71 @@ def downsample_segmentation_device(d_in: int, dtype: int, zyx, factor, d_workspa
     zyx, f = _zyx_and_factor(zyx, factor)
     _check_refusal(load().cfb_downsample_segmentation_device(C.c_void_p(d_in), int(dtype), *zyx, C.byref(f),
                                                              C.c_void_p(d_workspace or None), C.c_void_p(d_out), C.c_void_p(stream)))
+
+
+# ---- `gaussian-filter` and the median filter (include/chunkflow_b200.h, DESIGN.md section 0, row f8) ----
+FILTER_DTYPES = (DTYPE_U8, DTYPE_F32)
+FILTER_MODES = {"reflect": 0, "grid-mirror": 0, "nearest": 1, "mirror": 2, "wrap": 3, "grid-wrap": 3, "constant": 4,
+                "grid-constant": 4}
+MAX_GAUSSIAN_RADIUS = 64
+MAX_MEDIAN_WINDOW = 125
+
+
+def _czyx(shape):
+    shape = tuple(int(v) for v in shape)
+    if len(shape) not in (3, 4) or min(shape) <= 0:
+        raise ValueError(f"a chunk is (z, y, x) or (c, z, y, x) with positive sizes, not {shape}")
+    return (1,) + shape if len(shape) == 3 else shape
+
+
+def _filter_dtype(dtype: int) -> int:
+    if dtype not in FILTER_DTYPES:
+        raise TypeError("the filters take DTYPE_U8 or DTYPE_F32 chunks")
+    return int(dtype)
+
+
+def gaussian_filter_workspace(dtype: int, shape) -> int:
+    """Bytes of device workspace cfb_gaussian_filter_device needs for a chunk of ``shape`` (no device needed)."""
+    dtype, czyx, out = _filter_dtype(dtype), _czyx(shape), C.c_int64()
+    check(load().cfb_gaussian_filter_workspace(dtype, *czyx, C.byref(out)))
+    return int(out.value)
+
+
+def gaussian_filter_device(d_data: int, dtype: int, shape, weights, d_workspace: int, workspace_bytes: int, stream: int = 0) -> None:
+    """In place: every z section of the (z, y, x) or (c, z, y, x) chunk at ``d_data`` filtered along c (4-D only), y and x
+    with ``weights`` = one float64 array w[0..r] per axis (w[0] the centre) or None where the axis has no pass."""
+    dtype, czyx = _filter_dtype(dtype), _czyx(shape)
+    weights = list(weights)
+    if len(weights) != (3 if len(tuple(shape)) == 4 else 2):
+        raise ValueError("one weight array (or None) per axis of a section")
+    if len(weights) == 2:
+        weights = [None] + weights
+    args, keep = [], []
+    for w in weights:
+        if w is None:
+            args += [None, 0]
+            continue
+        w = np.ascontiguousarray(w, dtype=np.float64)
+        if w.ndim != 1 or not 1 <= w.size <= MAX_GAUSSIAN_RADIUS + 1:
+            raise ValueError(f"gaussian filter: a radius of {w.size - 1} exceeds the limit of {MAX_GAUSSIAN_RADIUS}")
+        keep.append(w)
+        args += [w.ctypes.data_as(C.POINTER(C.c_double)), w.size - 1]
+    check(load().cfb_gaussian_filter_device(C.c_void_p(d_data), dtype, *czyx, *args, C.c_void_p(d_workspace),
+                                            int(workspace_bytes), C.c_void_p(stream)))
+
+
+def median_filter_device(d_in: int, dtype: int, shape, size, mode: str, d_out: int, stream: int = 0) -> None:
+    """``d_out`` = the median filter of the (z, y, x) or (c, z, y, x) chunk at ``d_in`` with the window ``size`` (one extent
+    per axis of the chunk) and boundary ``mode`` (a scipy.ndimage mode name)."""
+    ndim, dtype, czyx = len(tuple(shape)), _filter_dtype(dtype), _czyx(shape)
+    size = tuple(int(v) for v in size)
+    if len(size) != ndim:
+        raise ValueError("one window extent per axis of the chunk")
+    if mode not in FILTER_MODES:
+        raise ValueError(f"unknown mode {mode}")
+    s = (C.c_int64 * 4)(*((1,) + size if ndim == 3 else size))
+    check(load().cfb_median_filter_device(C.c_void_p(d_in), dtype, *czyx, C.byref(s), FILTER_MODES[mode],
+                                          C.c_void_p(d_out), C.c_void_p(stream)))
 
 
 def device_memory(device: int = 0) -> tuple:

@@ -226,6 +226,16 @@ class Chunk(NDArrayOperatorsMixin):
         dev = DeviceChunk.from_chunk(self)
         return dev.connected_component(threshold=threshold, connectivity=connectivity).to_chunk()
 
+    def gaussian_filter_2d(self, sigma=1, device="cuda:0") -> None:
+        """Gaussian blur of every z section in place (reference chunk/base.py:846-853: ``gaussian_filter(array[..., z, :, :],
+        sigma)`` for every z), bit-identical to scipy.ndimage.  On a (c,z,y,x) chunk the section is the (c,y,x) block, so the
+        blur also runs across the channels, as in the reference.  It runs on the GPU (DeviceChunk.gaussian_filter_2d) and the
+        result is written back into this chunk's array, so views of it see the change; there is no CPU fallback."""
+        from .device import DeviceChunk
+        dev = DeviceChunk.from_chunk(self, device=device)
+        dev.gaussian_filter_2d(sigma)
+        self.array[...] = dev.tensor.cpu().numpy()
+
     def mask_using_last_channel(self, threshold: float = 0.3) -> "Chunk":
         """Drop the last channel and zero where it is >= threshold (reference base.py:685-689)."""
         keep = self.array[-1] < threshold

@@ -14,6 +14,8 @@ bookkeeping of the reference's ``Chunk`` and mirrors, name for name, the referen
     evaluate             reference chunk/segmentation.py:33-67          (Segmentation -> gala, lib/gala/evaluate.py)
     remap, mask_fragments, mask_except
                          reference chunk/segmentation.py:69-109         (Segmentation -> fastremap)
+    gaussian_filter_2d   reference chunk/base.py:846-853                (Chunk -> scipy.ndimage.gaussian_filter)
+    median_filter        reference plugins/median_filter.py:4-7         (plugin -> scipy.ndimage.median_filter)
 
 so that ``create-chunk | normalize-contrast | inference | crop-margin | quantize`` moves the image to the GPU once and
 brings a uint8 thumbnail (or nothing) back instead of the 12-byte-per-voxel affinity map.  There is no CPU fallback.
@@ -94,6 +96,37 @@ def selected_ids(selected_obj_ids) -> Optional[np.ndarray]:
     if any(not -2 ** 63 <= i < 2 ** 64 for i in ids):
         raise ValueError("a selected id does not fit in 64 bits")
     return np.array([i % 2 ** 64 for i in ids], dtype=np.uint64)
+
+
+def gaussian_weights(sigma) -> np.ndarray:
+    """float64 weights w[0..radius] (w[0] the centre) of scipy.ndimage's gaussian kernel at truncate 4.  Computed here with
+    numpy, with scipy's own expression, and handed to the kernel: numpy's exp and the C library's may differ in the last bit,
+    and one bit in a weight can change a truncated uint8 result."""
+    sigma = float(sigma)
+    radius = int(4.0 * sigma + 0.5)
+    x = np.arange(-radius, radius + 1)
+    w = np.exp(-0.5 / sigma ** 2 * x ** 2)
+    w = w / w.sum()
+    return np.ascontiguousarray(w[radius:])
+
+
+def _per_axis(value, ndim, kind=float) -> list:
+    """A scalar or one value per axis, like scipy.ndimage's _normalize_sequence (RuntimeError on another length)."""
+    v = np.asarray(value)
+    if v.ndim == 0:
+        return [kind(v)] * ndim
+    if v.ndim != 1 or v.size != ndim:
+        raise RuntimeError("sequence argument must have length equal to input rank")
+    return [kind(e) for e in v]
+
+
+def _filter_code(t) -> int:
+    torch = _torch()
+    if t.dtype == torch.uint8:
+        return _native.DTYPE_U8
+    if t.dtype == torch.float32:
+        return _native.DTYPE_F32
+    raise TypeError(f"the filters take uint8 or float32 chunks, not {t.dtype}")
 
 
 def _grown_table(device, slots: int, workspace_bytes, build, what: str):
@@ -525,6 +558,56 @@ class DeviceChunk:
         fc = Cartesian(*f)
         return DeviceChunk(out, voxel_offset=self.voxel_offset // fc,
                            voxel_size=None if self.voxel_size is None else self.voxel_size * fc, layer_type=self.layer_type)
+
+    # ---- Chunk.gaussian_filter_2d, plugins/median_filter.py ----------------------------------------------------------
+    def gaussian_filter_2d(self, sigma=1, per_channel: bool = False) -> None:
+        """In place, like the reference's Chunk.gaussian_filter_2d (chunk/base.py:846-853): for every z,
+        ``scipy.ndimage.gaussian_filter(array[..., z, :, :], sigma)`` bit for bit (csrc/filter_kernels.cuh).  On a (c,z,y,x)
+        chunk that section is the (c,y,x) block, so -- as in the reference -- the blur also runs across the channels, the
+        channel axis reflected like the others; ``sigma`` is then a scalar or (c, y, x), on a (z,y,x) chunk a scalar or (y, x).
+        ``per_channel=True`` filters every (y,x) plane on its own instead, as plugins/gaussian_filter.py does.  An axis with
+        sigma <= 1e-15 is not filtered.  uint8 or float32; a radius int(4 sigma + 0.5) above 64 raises ValueError, another
+        dtype TypeError, before any kernel runs."""
+        torch = _torch()
+        t = self.tensor
+        code = _filter_code(t)
+        axes = 2 if t.ndim == 3 or per_channel else 3
+        weights = []
+        for s in _per_axis(sigma, axes):
+            w = gaussian_weights(s) if s > 1e-15 else None
+            if w is not None and len(w) - 1 > _native.MAX_GAUSSIAN_RADIUS:
+                raise ValueError(f"gaussian filter: radius {len(w) - 1} exceeds the limit of {_native.MAX_GAUSSIAN_RADIUS}")
+            weights.append(w)
+        if t.ndim == 4 and per_channel:
+            weights = [None] + weights
+        with self._on_device():
+            work_bytes = _native.gaussian_filter_workspace(code, t.shape)
+            work = torch.empty(work_bytes, dtype=torch.uint8, device=t.device)
+            _native.gaussian_filter_device(t.data_ptr(), code, t.shape, weights, work.data_ptr(), work_bytes, self._stream())
+            del work   # the caching allocator keeps it for the stream until the kernels have run
+
+    def median_filter(self, size=(3, 1, 1), mode: str = "reflect") -> "DeviceChunk":
+        """``scipy.ndimage.median_filter(array, size=size, mode=mode)`` bit for bit, as plugins/median_filter.py runs it
+        (csrc/filter_kernels.cuh): element V // 2 of the sorted window of V elements, the window of extent s spanning offsets
+        -(s // 2) .. s - 1 - (s // 2).  ``size`` is a scalar or one extent per axis of the chunk (RuntimeError otherwise,
+        like scipy); ``mode`` reflect, nearest, mirror, wrap, constant (0) or a grid-* alias.  uint8 or float32, windows of at
+        most 125 elements.  Returns a new chunk with the same offset, voxel size and layer type.  float32 NaN and the sign of
+        a zero in a tie are outside the bit-identity claim."""
+        torch = _torch()
+        t = self.tensor
+        code = _filter_code(t)
+        extents = _per_axis(size, t.ndim, int)
+        if mode not in _native.FILTER_MODES:
+            raise RuntimeError(f"boundary mode not supported: {mode}")
+        if min(extents) < 1:
+            raise ValueError("every window extent must be at least 1")
+        volume = int(np.prod(extents))
+        if volume > _native.MAX_MEDIAN_WINDOW:
+            raise ValueError(f"median filter: a window of {volume} elements exceeds the limit of {_native.MAX_MEDIAN_WINDOW} (5x5x5)")
+        out = torch.empty_like(t)
+        with self._on_device():
+            _native.median_filter_device(t.data_ptr(), code, t.shape, extents, mode, out.data_ptr(), self._stream())
+        return DeviceChunk(out, voxel_offset=self.voxel_offset, voxel_size=self.voxel_size, layer_type=self.layer_type)
 
     def __repr__(self):
         return f"DeviceChunk(shape={self.shape}, dtype={self.dtype}, voxel_offset={tuple(self.voxel_offset)}, device={self.tensor.device})"

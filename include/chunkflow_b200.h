@@ -27,6 +27,9 @@
  *   cfb_label_table_*, cfb_label_apply_device
  *                                 Segmentation.remap / mask_fragments / mask_except   chunk/segmentation.py:69-109
  *   cfb_downsample_*              the `downsample` command   flow/flow.py:1545-1573 (-> lib/igneous/downsample.py)
+ *   cfb_gaussian_filter_*         Chunk.gaussian_filter_2d   chunk/base.py:846-853 (`gaussian-filter`, flow/flow.py:1615-1630),
+ *                                 plugins/gaussian_filter.py:7-23 (-> scipy.ndimage.gaussian_filter)
+ *   cfb_median_filter_device      plugins/median_filter.py:4-7 (-> scipy.ndimage.median_filter)
  *
  * Plain pointers and sizes only -- no torch types.  Device pointers are raw CUDA device
  * addresses (e.g. torch.Tensor.data_ptr()) owned by the caller.  All functions return
@@ -431,6 +434,39 @@ int cfb_downsample_workspace(int32_t dtype, int64_t z, int64_t y, int64_t x, con
                              int64_t* workspace_bytes);
 int cfb_downsample_segmentation_device(const void* d_in, int32_t dtype, int64_t z, int64_t y, int64_t x, const int64_t factor[3],
                                        void* d_workspace, void* d_out, void* stream);
+
+/* `gaussian-filter` and the median filter (DESIGN.md section 0, row f8): the reference calls scipy.ndimage.gaussian_filter
+ * (Chunk.gaussian_filter_2d, chunk/base.py:846-853; plugins/gaussian_filter.py:7-23) and scipy.ndimage.median_filter
+ * (plugins/median_filter.py:4-7); the results here are bit-identical to scipy's on uint8 and float32, restated in
+ * oracle/filters_oracle.py.  The chunk is (c, z, y, x) C-order, c = 1 for a 3-D chunk; dtype CFB_DTYPE_U8 or CFB_DTYPE_F32.
+ *
+ * cfb_gaussian_filter_device  in place: every z section is filtered on its own, one 1-D pass per axis in the order c, y, x;
+ *     the channel pass mixes the channels of a section, as the reference does on a 4-D chunk.  w_<axis>[0..r_<axis>] are the
+ *     float64 weights of scipy's kernel at truncate 4, w[0] the centre: radius r = int(4 sigma + 0.5),
+ *     w = exp(-0.5 / sigma^2 * k^2) for k = -r..r, divided by their sum -- computed by the CALLER with numpy (numpy's and
+ *     libm's exp may differ in the last bit).  A null w_<axis> with r_<axis> = 0 means no pass along that axis (scipy skips
+ *     sigma <= 1e-15).  Per element, in float64, every operation rounded on its own: t = x[i] * w[0], then
+ *     t = t + (x[i-j] + x[i+j]) * w[j] for j = r .. 1, indices reflected (d c b a | a b c d | d c b a, period 2n); then a cast
+ *     to the chunk's type (uint8: toward zero, float32: to nearest) that the next pass reads.  r is 0 .. 64.
+ *     d_workspace: cfb_gaussian_filter_workspace bytes (a batch of whole sections), not overlapping the chunk.
+ * cfb_median_filter_device  out = element V / 2 of the sorted window of V = prod(size) elements (at most 125; each extent
+ *     1 .. 125); the window of extent s spans offsets -(s / 2) .. s - 1 - (s / 2).  mode: CFB_FILTER_REFLECT (scipy 'reflect',
+ *     'grid-mirror'), _NEAREST, _MIRROR (d c b | a b c d | c b a; one element mirrors onto itself), _WRAP ('wrap',
+ *     'grid-wrap'), _CONSTANT (the value 0; 'constant', 'grid-constant').  size (1, 3, 1, 1) -- scipy's (3, 1, 1) on a 3-D
+ *     chunk -- reads the chunk once.  Input and output must not overlap.  Outside the bit-identity claim: float32 NaN, and
+ *     the sign of a zero in a tie of +0 and -0.
+ * Sizes, radii and windows out of range return CFB_ERR_INVALID_ARGUMENT before any kernel runs.  64-bit indices; any address. */
+#define CFB_FILTER_REFLECT 0
+#define CFB_FILTER_NEAREST 1
+#define CFB_FILTER_MIRROR 2
+#define CFB_FILTER_WRAP 3
+#define CFB_FILTER_CONSTANT 4
+int cfb_gaussian_filter_workspace(int32_t dtype, int64_t c, int64_t z, int64_t y, int64_t x, int64_t* workspace_bytes);
+int cfb_gaussian_filter_device(void* d_data, int32_t dtype, int64_t c, int64_t z, int64_t y, int64_t x, const double* w_c,
+                               int32_t r_c, const double* w_y, int32_t r_y, const double* w_x, int32_t r_x, void* d_workspace,
+                               int64_t workspace_bytes, void* stream);
+int cfb_median_filter_device(const void* d_in, int32_t dtype, int64_t c, int64_t z, int64_t y, int64_t x, const int64_t size[4],
+                             int32_t mode, void* d_out, void* stream);
 
 #ifdef __cplusplus
 }
