@@ -36,6 +36,7 @@ EXPORTS = (
     "cfb_label_table_workspace", "cfb_label_table_device", "cfb_label_table_read", "cfb_label_table_plan",
     "cfb_label_apply_device", "cfb_downsample_average_device", "cfb_downsample_workspace", "cfb_downsample_segmentation_device",
     "cfb_gaussian_filter_workspace", "cfb_gaussian_filter_device", "cfb_median_filter_device",
+    "cfb_clahe_workspace", "cfb_clahe_device",
 )
 
 
@@ -165,6 +166,8 @@ def load() -> C.CDLL:
     lib.cfb_gaussian_filter_workspace.argtypes = [i32, i64, i64, i64, i64, C.POINTER(i64)]
     lib.cfb_gaussian_filter_device.argtypes = [vp, i32, i64, i64, i64, i64, dp, i32, dp, i32, dp, i32, vp, i64, vp]
     lib.cfb_median_filter_device.argtypes = [vp, i32, i64, i64, i64, i64, C.POINTER(i64 * 4), i32, vp, vp]
+    lib.cfb_clahe_workspace.argtypes = [i64, i64, i64, i32, i32, C.POINTER(i64)]
+    lib.cfb_clahe_device.argtypes = [vp, vp, i64, i64, i64, C.c_double, i32, i32, vp, i64, vp]
     for name in EXPORTS:
         getattr(lib, name)   # every declared symbol must be there
     _lib = lib
@@ -517,6 +520,35 @@ def median_filter_device(d_in: int, dtype: int, shape, size, mode: str, d_out: i
     s = (C.c_int64 * 4)(*((1,) + size if ndim == 3 else size))
     check(load().cfb_median_filter_device(C.c_void_p(d_in), dtype, *czyx, C.byref(s), FILTER_MODES[mode],
                                           C.c_void_p(d_out), C.c_void_p(stream)))
+
+
+# ---- `clahe` (include/chunkflow_b200.h, DESIGN.md section 0, row f9) ----
+def clahe_args(shape, tile_grid_size) -> tuple:
+    """((z, y, x), tiles_x, tiles_y) of a clahe call; ValueError for another ndim or fewer than one tile along an axis."""
+    shape = tuple(int(v) for v in shape)
+    if len(shape) != 3 or min(shape) <= 0:
+        raise ValueError(f"clahe takes a (z, y, x) image with positive sizes, not {shape}")
+    tiles = tuple(int(v) for v in tile_grid_size)
+    if len(tiles) != 2 or min(tiles) < 1:
+        raise ValueError(f"the tile grid (x, y) has at least one tile along each axis, not {tile_grid_size}")
+    return shape, tiles[0], tiles[1]
+
+
+def clahe_workspace(shape, tile_grid_size) -> int:
+    """Bytes of device workspace cfb_clahe_device needs for a (z, y, x) chunk and an (x, y) tile grid (no device needed)."""
+    zyx, tx, ty = clahe_args(shape, tile_grid_size)
+    out = C.c_int64()
+    check(load().cfb_clahe_workspace(*zyx, tx, ty, C.byref(out)))
+    return int(out.value)
+
+
+def clahe_device(d_in: int, d_out: int, shape, clip_limit: float, tile_grid_size, d_workspace: int, workspace_bytes: int,
+                 stream: int = 0) -> None:
+    """``d_out`` = cv2.createCLAHE(clip_limit, tile_grid_size).apply of every z section of the uint8 (z, y, x) chunk at
+    ``d_in``; tile_grid_size is (x, y), cv2's order."""
+    zyx, tx, ty = clahe_args(shape, tile_grid_size)
+    check(load().cfb_clahe_device(C.c_void_p(d_in), C.c_void_p(d_out), *zyx, float(clip_limit), tx, ty,
+                                  C.c_void_p(d_workspace or None), int(workspace_bytes), C.c_void_p(stream)))
 
 
 def device_memory(device: int = 0) -> tuple:

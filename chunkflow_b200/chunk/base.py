@@ -160,6 +160,11 @@ class Chunk(NDArrayOperatorsMixin):
     def voxel_stop(self) -> tuple:
         return tuple(o + s for o, s in zip(self.ndoffset, self.shape))
 
+    @property
+    def is_image(self) -> bool:
+        """uint8 and 3-D (reference chunk/base.py:495-497)."""
+        return self.array.dtype == np.uint8 and self.array.ndim == 3
+
     # ---- layer type guess (lazy) ---------------------------------------------------
     @property
     def layer_type(self) -> str:

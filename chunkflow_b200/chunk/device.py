@@ -16,6 +16,7 @@ bookkeeping of the reference's ``Chunk`` and mirrors, name for name, the referen
                          reference chunk/segmentation.py:69-109         (Segmentation -> fastremap)
     gaussian_filter_2d   reference chunk/base.py:846-853                (Chunk -> scipy.ndimage.gaussian_filter)
     median_filter        reference plugins/median_filter.py:4-7         (plugin -> scipy.ndimage.median_filter)
+    clahe                reference plugins/clahe.py                     (plugin -> cv2.createCLAHE(...).apply)
 
 so that ``create-chunk | normalize-contrast | inference | crop-margin | quantize`` moves the image to the GPU once and
 brings a uint8 thumbnail (or nothing) back instead of the 12-byte-per-voxel affinity map.  There is no CPU fallback.
@@ -186,6 +187,11 @@ class DeviceChunk:
     @property
     def dtype(self):
         return self.tensor.dtype
+
+    @property
+    def is_image(self) -> bool:
+        """uint8 and 3-D, like the reference's Chunk.is_image."""
+        return self.tensor.dtype == _torch().uint8 and self.tensor.ndim == 3
 
     def _czyx(self):
         s = self.shape
@@ -607,6 +613,26 @@ class DeviceChunk:
         out = torch.empty_like(t)
         with self._on_device():
             _native.median_filter_device(t.data_ptr(), code, t.shape, extents, mode, out.data_ptr(), self._stream())
+        return DeviceChunk(out, voxel_offset=self.voxel_offset, voxel_size=self.voxel_size, layer_type=self.layer_type)
+
+    # ---- plugins/clahe.py ------------------------------------------------------------------------------------------------
+    def clahe(self, clip_limit: float = 20.0, tile_grid_size=(512, 512)) -> "DeviceChunk":
+        """``cv2.createCLAHE(clip_limit, tile_grid_size).apply`` of every z section bit for bit, as plugins/clahe.py runs it
+        (csrc/clahe_kernels.cuh).  ``tile_grid_size`` is (x, y) -- OpenCV's order, x first.  A clip limit <= 0 means no
+        clipping.  uint8 (z, y, x) only: another dtype raises TypeError, another ndim or fewer than one tile along an axis
+        ValueError, before any kernel runs.  Returns a new chunk with the same offset, voxel size and layer type."""
+        torch = _torch()
+        t = self.tensor
+        if t.dtype != torch.uint8:
+            raise TypeError(f"clahe takes uint8 images, not {t.dtype}")
+        zyx, tx, ty = _native.clahe_args(t.shape, tile_grid_size)
+        out = torch.empty_like(t)
+        with self._on_device():
+            work_bytes = _native.clahe_workspace(zyx, (tx, ty))
+            work = torch.empty(work_bytes, dtype=torch.uint8, device=t.device) if work_bytes else None
+            _native.clahe_device(t.data_ptr(), out.data_ptr(), zyx, clip_limit, (tx, ty), work.data_ptr() if work_bytes else 0,
+                                 work_bytes, self._stream())
+            del work   # the caching allocator keeps it for the stream until the kernels have run
         return DeviceChunk(out, voxel_offset=self.voxel_offset, voxel_size=self.voxel_size, layer_type=self.layer_type)
 
     def __repr__(self):

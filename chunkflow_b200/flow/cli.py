@@ -368,6 +368,30 @@ def median_filter(tasks, input_chunk_name, output_chunk_name, size, mode):
         yield task
 
 
+@main.command("clahe")
+@click.option("--input-chunk-name", "-i", type=str, default="chunk", help="input chunk name")
+@click.option("--output-chunk-name", "-o", type=str, default="chunk", help="output chunk name")
+@click.option("--clip-limit", "-c", type=click.FLOAT, default=20.0, help="contrast limit; 0 or less: no clipping.")
+@click.option("--tile-grid-size", "-t", type=click.INT, nargs=2, default=(512, 512),
+              help="number of tiles in x and y (OpenCV's order, x first).")
+@operator
+def clahe(tasks, input_chunk_name, output_chunk_name, clip_limit, tile_grid_size):
+    """(extension) Contrast-limited adaptive histogram equalization of every z section of a uint8 image, bit-identical to
+    cv2.createCLAHE(clip_limit, tile_grid_size).apply: the reference runs it as `plugin -f clahe` (plugins/clahe.py).
+    A host chunk comes back to the host, a GPU-resident one stays there."""
+    import torch
+    for task in tasks:
+        if task is not None:
+            dev, was_host = _on_device(task[input_chunk_name], "cuda:0")
+            out = dev.clahe(clip_limit, tile_grid_size)
+            torch.cuda.synchronize(out.tensor.device)
+            if was_host:
+                out = Chunk(out.to_chunk().array, voxel_offset=out.voxel_offset, voxel_size=out.voxel_size,
+                            layer_type=getattr(task[input_chunk_name], "_layer_type", None))
+            task[output_chunk_name] = out
+        yield task
+
+
 @main.command("evaluate-segmentation")
 @click.option("--segmentation-chunk-name", "-s", type=str, default="chunk", help="chunk name of segmentation")
 @click.option("--groundtruth-chunk-name", "-g", type=str, default="groundtruth")

@@ -30,6 +30,7 @@
  *   cfb_gaussian_filter_*         Chunk.gaussian_filter_2d   chunk/base.py:846-853 (`gaussian-filter`, flow/flow.py:1615-1630),
  *                                 plugins/gaussian_filter.py:7-23 (-> scipy.ndimage.gaussian_filter)
  *   cfb_median_filter_device      plugins/median_filter.py:4-7 (-> scipy.ndimage.median_filter)
+ *   cfb_clahe_*                   plugins/clahe.py (-> cv2.createCLAHE(clipLimit, tileGridSize).apply)
  *
  * Plain pointers and sizes only -- no torch types.  Device pointers are raw CUDA device
  * addresses (e.g. torch.Tensor.data_ptr()) owned by the caller.  All functions return
@@ -467,6 +468,29 @@ int cfb_gaussian_filter_device(void* d_data, int32_t dtype, int64_t c, int64_t z
                                int64_t workspace_bytes, void* stream);
 int cfb_median_filter_device(const void* d_in, int32_t dtype, int64_t c, int64_t z, int64_t y, int64_t x, const int64_t size[4],
                              int32_t mode, void* d_out, void* stream);
+
+/* `clahe` (DESIGN.md section 0, row f9): the reference's plugins/clahe.py runs cv2.createCLAHE(clipLimit, tileGridSize).apply
+ * on every z section of a uint8 image; the results here are bit-identical to OpenCV's, restated in oracle/clahe_oracle.py.
+ * The chunk is uint8 (z, y, x) C-order; every section is equalized on its own.  tiles_x, tiles_y: cv2's tileGridSize, x first.
+ *   padding   none when x % tiles_x == 0 and y % tiles_y == 0, else tiles_y - y % tiles_y rows at the bottom and
+ *             tiles_x - x % tiles_x columns at the right (OpenCV pads both), BORDER_REFLECT_101 (d c b | a b c d | c b a),
+ *             tiles of th x tw = T pixels of the padded section;
+ *   clipping  clip_limit > 0: cl = max((int)(clip_limit * T / 256), 1) in double (out of the int32 range: INT32_MIN, as x86
+ *             casts, so cl = 1); each tile's 256-bin histogram is clipped at cl, the clipped count spread over the bins
+ *             (count / 256 to every bin, one more to bins 0, step, 2 step, ... while count % 256 lasts,
+ *             step = max(256 / (count % 256), 1)).  clip_limit <= 0: no clipping;
+ *   LUT       lut[v] = sat_u8(rint(float(cumsum(v)) * (255.f / T)));
+ *   output    float32, every operation rounded on its own: txf = x * (1.f / tw) - 0.5f, tx1 = floor(txf), xa = txf - tx1,
+ *             tx2 = min(tx1 + 1, tiles_x - 1), tx1 = max(tx1, 0), the same along y, and
+ *             sat_u8(rint((L11 (1 - xa) + L12 xa) (1 - ya) + (L21 (1 - xa) + L22 xa) ya)), Lab = lut of tile (ty_a, tx_b).
+ * cfb_clahe_workspace  bytes of d_workspace (the tile LUTs of a batch of sections; 0 for tiles of at most 64 pixels, whose
+ *     LUT entries are computed where they are read).  No device needed.
+ * cfb_clahe_device  d_out must not overlap d_in, nor the workspace either.  A section side above 2^24 pixels, a padded section
+ *     above INT32_MAX pixels, or tiles_x / tiles_y below 1 return CFB_ERR_INVALID_ARGUMENT before any kernel runs.
+ *     64-bit indices; any address. */
+int cfb_clahe_workspace(int64_t z, int64_t y, int64_t x, int32_t tiles_x, int32_t tiles_y, int64_t* workspace_bytes);
+int cfb_clahe_device(const void* d_in, void* d_out, int64_t z, int64_t y, int64_t x, double clip_limit, int32_t tiles_x,
+                     int32_t tiles_y, void* d_workspace, int64_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
