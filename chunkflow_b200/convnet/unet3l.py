@@ -1,4 +1,4 @@
-"""Canonical 3-level 3D U-Net for the ``inference`` hot path (SURVEY.md section 7.2).
+"""The plain 3D U-Net family for the ``inference`` hot path (SURVEY.md section 7.2).
 
 The reference ships no network definition: ``-f pytorch`` loads a user file that must
 expose ``load_model(weight_path)`` or ``InstantiatedModel`` (plus optional
@@ -7,13 +7,14 @@ expose ``load_model(weight_path)`` or ``InstantiatedModel`` (plus optional
 contract, so the SAME file drives
 
 * the reference's own ``-f pytorch`` CPU path (the parity oracle), and
-* the device path, which reads :data:`LAYER_SPEC` / the ``state_dict`` and packs the
-  weights into the device layout of the hand-written sm_90a kernels.
+* the device path, which reads the ``state_dict`` (its depth from the ``enc{k}.0`` names)
+  and packs the weights into the device layout of the hand-written sm_90a kernels.
 
 It must stay self-contained (no package-relative imports): the reference executes it
 through ``SourceFileLoader("Model", fname)`` (``chunkflow/lib/__init__.py:5-16``).
 
-Architecture (fixed): widths (16, 32, 64), pooling (1, 2, 2)
+Architecture: depth d in {2, 3, 4}, widths (16, 32, ..., 16 * 2**(d-1)), pooling (1, 2, 2).
+Depth 3 (:class:`UNet3L`, the default) is
 
     enc0: conv3x3x3(1->16)+ReLU, conv3x3x3(16->16)+ReLU          full resolution
     pool (1,2,2)
@@ -26,28 +27,57 @@ Architecture (fixed): widths (16, 32, 64), pooling (1, 2, 2)
     dec0: conv3x3x3(32->16)+ReLU, conv3x3x3(16->16)+ReLU
     head: conv1x1x1(16->cout) + sigmoid
 
+Depth 2 stops after enc1; depth 4 adds enc3 (64->128, 128->128, 1/8 in y,x), up2 (128->64)
+and dec2 (128->64, 64->64).  Patch y and x must be multiples of 2**(d-1).
 All 3x3x3 convolutions use zero padding 1 (SAME) at the *patch* border.
-141 248 FLOP per patch voxel for cout=3.
+FLOP per patch voxel for cout=3 (:func:`flops_per_voxel`): 78 016 (depth 2), 141 248 (depth 3),
+204 480 (depth 4).  This is not RSUNet: no residual blocks, no normalisation.
 """
 import math
 
 import torch
 import torch.nn as nn
 
-WIDTHS = (16, 32, 64)
+DEPTHS = (2, 3, 4)
 POOL = (1, 2, 2)
 
-# (name, kind, cin, cout) in execution order; the device path packs weights by name.
-LAYER_SPEC = (
-    ("enc0.0", "conv3", 1, 16), ("enc0.2", "conv3", 16, 16),
-    ("enc1.0", "conv3", 16, 32), ("enc1.2", "conv3", 32, 32),
-    ("enc2.0", "conv3", 32, 64), ("enc2.2", "conv3", 64, 64),
-    ("up1", "convT", 64, 32),
-    ("dec1.0", "conv3", 64, 32), ("dec1.2", "conv3", 32, 32),
-    ("up0", "convT", 32, 16),
-    ("dec0.0", "conv3", 32, 16), ("dec0.2", "conv3", 16, 16),
-    ("head", "conv1", 16, None),
-)
+
+def widths(depth: int = 3) -> tuple:
+    """Channels of the levels: 16, 32, ... doubling with every (1,2,2) pool."""
+    return tuple(16 << k for k in range(depth))
+
+
+WIDTHS = widths(3)
+
+
+def layer_spec(depth: int = 3) -> tuple:
+    """(name, kind, cin, cout) in execution order; the device path generates the same table from the state dict."""
+    w = widths(depth)
+    spec = []
+    for k in range(depth):
+        spec += [(f"enc{k}.0", "conv3", w[k - 1] if k else 1, w[k]), (f"enc{k}.2", "conv3", w[k], w[k])]
+    for k in range(depth - 2, -1, -1):
+        spec += [(f"up{k}", "convT", w[k + 1], w[k]),
+                 (f"dec{k}.0", "conv3", 2 * w[k], w[k]), (f"dec{k}.2", "conv3", w[k], w[k])]
+    spec.append(("head", "conv1", w[0], None))
+    return tuple(spec)
+
+
+# the default (3-level) network's layers
+LAYER_SPEC = layer_spec(3)
+
+
+def flops_per_voxel(depth: int = 3, cout: int = 3) -> int:
+    """Algorithmic FLOP (2 per multiply-add) per input patch voxel; the max pools are not counted."""
+    total = 0
+    for name, kind, ci, co in layer_spec(depth):
+        if kind == "conv1":
+            total += 2 * ci * cout
+            continue
+        level = int(name[3]) if name.startswith(("enc", "dec")) else int(name[2:])
+        taps = 27 if kind == "conv3" else 1  # a transposed convolution: one tap per output voxel (at its output level)
+        total += 2 * taps * ci * co * 4 ** (depth - 1 - level) // 4 ** (depth - 1)
+    return total
 
 
 def _block(cin, cout):
@@ -57,29 +87,41 @@ def _block(cin, cout):
     )
 
 
-class UNet3L(nn.Module):
-    def __init__(self, cin: int = 1, cout: int = 3):
+class UNet(nn.Module):
+    """Modules are registered enc0 .. enc{d-1}, up{d-2}, dec{d-2} .. up0, dec0, head, pool: the seeded
+    initialisation draws in this order."""
+
+    def __init__(self, cin: int = 1, cout: int = 3, depth: int = 3):
         super().__init__()
-        w0, w1, w2 = WIDTHS
-        self.enc0 = _block(cin, w0)
-        self.enc1 = _block(w0, w1)
-        self.enc2 = _block(w1, w2)
-        self.up1 = nn.ConvTranspose3d(w2, w1, kernel_size=POOL, stride=POOL)
-        self.dec1 = _block(2 * w1, w1)
-        self.up0 = nn.ConvTranspose3d(w1, w0, kernel_size=POOL, stride=POOL)
-        self.dec0 = _block(2 * w0, w0)
-        self.head = nn.Conv3d(w0, cout, 1)
+        if depth not in DEPTHS:
+            raise ValueError(f"U-Net depth must be one of {DEPTHS}, got {depth}")
+        self.depth = depth
+        w = widths(depth)
+        for k in range(depth):
+            setattr(self, f"enc{k}", _block(w[k - 1] if k else cin, w[k]))
+        for k in range(depth - 2, -1, -1):
+            setattr(self, f"up{k}", nn.ConvTranspose3d(w[k + 1], w[k], kernel_size=POOL, stride=POOL))
+            setattr(self, f"dec{k}", _block(2 * w[k], w[k]))
+        self.head = nn.Conv3d(w[0], cout, 1)
         self.pool = nn.MaxPool3d(POOL)
 
     def forward(self, x):
-        e0 = self.enc0(x)
-        e1 = self.enc1(self.pool(e0))
-        e2 = self.enc2(self.pool(e1))
-        d1 = self.dec1(torch.cat([self.up1(e2), e1], dim=1))
-        d0 = self.dec0(torch.cat([self.up0(d1), e0], dim=1))
+        enc = []
+        for k in range(self.depth):
+            x = getattr(self, f"enc{k}")(self.pool(x) if k else x)
+            enc.append(x)
+        for k in range(self.depth - 2, -1, -1):
+            x = getattr(self, f"dec{k}")(torch.cat([getattr(self, f"up{k}")(x), enc[k]], dim=1))
         # sigmoid is required: the reference asserts output < 1.0001
         # (chunkflow/flow/divid_conquer/inferencer.py:465-466)
-        return torch.sigmoid(self.head(d0))
+        return torch.sigmoid(self.head(x))
+
+
+class UNet3L(UNet):
+    """The 3-level member, widths (16, 32, 64)."""
+
+    def __init__(self, cin: int = 1, cout: int = 3):
+        super().__init__(cin, cout, depth=3)
 
 
 def seeded_init(model: nn.Module, seed: int = 0, head_gain: float = 4.0) -> nn.Module:
@@ -104,22 +146,38 @@ def seeded_init(model: nn.Module, seed: int = 0, head_gain: float = 4.0) -> nn.M
     return model
 
 
-def create_model(cin: int = 1, cout: int = 3, seed: int = 0) -> nn.Module:
-    return seeded_init(UNet3L(cin, cout), seed=seed).eval()
+def create_model(cin: int = 1, cout: int = 3, seed: int = 0, depth: int = 3) -> nn.Module:
+    return seeded_init(UNet(cin, cout, depth), seed=seed).eval()
+
+
+def state_depth(state) -> int:
+    """The depth of a state dict (its ``enc{k}.0.weight`` tensors), checked against the family: 2 to 4 levels,
+    level k ``16 << k`` channels wide."""
+    depth = 0
+    while f"enc{depth}.0.weight" in state:
+        depth += 1
+    if depth not in DEPTHS:
+        raise ValueError(f"U-Net depth must be one of {DEPTHS}: the checkpoint has {depth} encoder levels")
+    for k, w in enumerate(widths(depth)):
+        got = tuple(state[f"enc{k}.0.weight"].shape)[0]
+        if got != w:
+            raise ValueError(f"U-Net widths must double from 16 ({widths(depth)}): enc{k}.0 has {got} channels")
+    return depth
 
 
 def load_model(weight_path=None, cin: int = 1, cout: int = 3):
     """Entry point used by the reference ``-f pytorch`` loader (pytorch.py:50-51).
 
-    ``weight_path`` None/"" -> the seeded random init (there are no trained weights
-    offline); otherwise a ``state_dict`` or ``{'state_dict': ...}`` checkpoint.
+    ``weight_path`` None/"" -> the seeded random 3-level init (there are no trained weights
+    offline); otherwise a ``state_dict`` or ``{'state_dict': ...}`` checkpoint of any depth of the family.
     """
     if not weight_path:
         return create_model(cin, cout)
     chkpt = torch.load(weight_path, map_location="cpu")
     state = chkpt["state_dict"] if "state_dict" in chkpt else chkpt
+    depth = state_depth(state)
     cout = state["head.weight"].shape[0]
     cin = state["enc0.0.weight"].shape[1]
-    model = UNet3L(cin, cout)
+    model = UNet(cin, cout, depth)
     model.load_state_dict(state)
     return model.eval()

@@ -1,7 +1,8 @@
 // wgmma / TMA implicit-GEMM 3x3x3 convolution and the fp16 "chunk-planar" activation
 // layout it works on.  Declarations.
 //
-// Activation layout in HBM ("CP8"): (batch, C/8, P, Z, Y, X, 8) fp16, where P = 1 (single
+// Activation layout in HBM ("CP8"): (batch, C/8, P, Z, Y, X, 8) fp16 -- a tensor of 128 channels is stored half-major,
+// (2, batch, 8, P, Z, Y, X, 8), each 64-channel half a CP8 tensor of its own -- where P = 1 (single
 // fp16) or 2 (hi/lo split: value = hi + lo, |lo| <= ulp(hi)/2, ~22 significant bits).  One
 // (chunk, part) plane is a dense (Z, Y, X, 8) array of 16-byte voxel records, so that
 //   * TMA can stage a halo box of any (z, y, x) offset into shared memory with zero fill
@@ -13,6 +14,7 @@
 #pragma once
 #include <cuda_fp16.h>
 
+#include <array>
 #include <map>
 #include <memory>
 
@@ -38,6 +40,8 @@ struct PackedConv {
   float acc_scale = 1.0f;  // f16f8: 1 / (alpha * beta), applied to the accumulator by the epilogue
   size_t bytes = 0;
   std::shared_ptr<std::map<uint64_t, ConvTile>> tuned;  // chosen tiling per (size, batch)
+  // cout 128: no blocks of its own, but the two halves of 64 output channels, each packed as a layer (kernels_wgmma_wide.cu)
+  std::shared_ptr<std::array<PackedConv, 2>> halves;
 };
 
 void pack_conv3_weights(const float* h_w, const float* h_bias, int cin, int cout, int fmt, PackedConv& out);  // fmt: ActFmt
@@ -59,7 +63,7 @@ struct ConvTail {
   Int3 out_patch, crop, out_size;
   float scale;              // 1, or 1/8 when the batch holds the 8 test-time-augmentation variants
 };
-// `pool_out` (16->16 and 32->32 layers): the (1,2,2) max-pooled output, CP8 of (Z, Y/2, X/2), written by the same epilogue.
+// `pool_out` (16->16, 32->32 and 64->64 layers): the (1,2,2) max-pooled output, CP8 of (Z, Y/2, X/2), written by the same epilogue.
 void launch_conv3_wgmma(const __half* srcA, int ca, const __half* srcB, int cb, const PackedConv& w, __half* out,
                         int nb, Int3 size, bool relu, cudaStream_t s, const ConvTail* tail = nullptr, __half* pool_out = nullptr);
 // ConvTranspose kernel = stride = (1,2,2) on wgmma: in CP8 (nb, cin) of in_size, out CP8 (nb, cout) of (Z, 2Y, 2X); no ReLU.

@@ -210,7 +210,9 @@ convT_cp8_kernel(const uint4* __restrict__ in, const float* __restrict__ w, cons
     for (int co = 0; co < COUT; ++co) acc[co] = 0.f;
     for (int ch = 0; ch < ichunks; ++ch) {
       float v[8];
-      load8(in, ((size_t)b * ichunks + ch) * fmt_planes(parts), parts, ipvol, iv, v);
+      // 128 input channels are stored half-major (kernels_conv.cuh)
+      const size_t chunk = ichunks > 8 ? ((size_t)(ch >> 3) * nb + b) * 8 + (ch & 7) : (size_t)b * ichunks + ch;
+      load8(in, chunk * fmt_planes(parts), parts, ipvol, iv, v);
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
         const float* wp = &s_wt[((ch * 8 + e) * 4 + tap) * COUT];
@@ -352,10 +354,18 @@ void launch_convT_cp8(const __half* in, const float* w, const float* bias, __hal
   const size_t smem = (size_t)cin * cout * 4 * sizeof(float);
   auto in16 = reinterpret_cast<const uint4*>(in);
   auto out16 = reinterpret_cast<uint4*>(out);
-  if (cout == 32) {
-    convT_cp8_kernel<32><<<grid_for(items), kT, smem, s>>>(in16, w, bias, out16, cin, parts, nb, isz);
+  // the weights are staged as cin x cout x 4 floats: 128 KiB for the 128 -> 64 layer of the 4-level U-Net, above the
+  // 48 KiB a launch gets without opting in
+  auto launch = [&](auto kern) {
+    if (smem > 48 * 1024) CFB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid_for(items), kT, smem, s>>>(in16, w, bias, out16, cin, parts, nb, isz);
+  };
+  if (cout == 64) {
+    launch(convT_cp8_kernel<64>);
+  } else if (cout == 32) {
+    launch(convT_cp8_kernel<32>);
   } else if (cout == 16) {
-    convT_cp8_kernel<16><<<grid_for(items), kT, smem, s>>>(in16, w, bias, out16, cin, parts, nb, isz);
+    launch(convT_cp8_kernel<16>);
   } else {
     throw std::runtime_error("convT_cp8: unsupported cout");
   }

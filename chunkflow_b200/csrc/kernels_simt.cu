@@ -109,7 +109,7 @@ maxpool_f32_kernel(const float* __restrict__ in, float* __restrict__ out, int64_
   }
 }
 
-// One thread = one OUTPUT voxel, all output channels (<= 32).
+// One thread = one OUTPUT voxel, all output channels (<= 64).
 template <int COUT>
 __global__ void __launch_bounds__(256)
 convT_f32_kernel(const float* __restrict__ in, const float* __restrict__ w, const float* __restrict__ bias,
@@ -199,10 +199,18 @@ void launch_convT_f32(const float* in, const float* w, const float* bias, float*
                       Int3 isz, cudaStream_t s) {
   const int64_t items = (int64_t)nb * isz.z * isz.y * 2 * isz.x * 2;
   const size_t smem = (size_t)cin * cout * 4 * sizeof(float);
-  if (cout == 32) {
-    convT_f32_kernel<32><<<grid_for(items), 256, smem, s>>>(in, w, bias, out, cin, nb, isz);
+  // the weights are staged as cin x cout x 4 floats: 128 KiB for the 128 -> 64 layer of the 4-level U-Net, above the
+  // 48 KiB a launch gets without opting in
+  auto launch = [&](auto kern) {
+    if (smem > 48 * 1024) CFB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<grid_for(items), 256, smem, s>>>(in, w, bias, out, cin, nb, isz);
+  };
+  if (cout == 64) {
+    launch(convT_f32_kernel<64>);
+  } else if (cout == 32) {
+    launch(convT_f32_kernel<32>);
   } else if (cout == 16) {
-    convT_f32_kernel<16><<<grid_for(items), 256, smem, s>>>(in, w, bias, out, cin, nb, isz);
+    launch(convT_f32_kernel<16>);
   } else {
     throw std::runtime_error("convT_f32: unsupported cout");
   }

@@ -1,4 +1,4 @@
-// Device-side 3-level U-Net: weight packing, workspace and layer dispatch.
+// Device-side U-Net of depth 2 to 4: the generated layer table, weight packing, workspace and layer dispatch.
 #include "network.cuh"
 
 #include <cstdlib>
@@ -9,43 +9,43 @@
 
 namespace cfb {
 
-namespace {
-enum Op { kOpFirst, kOpConv3, kOpConv3Pool, kOpConvT, kOpHead };
-struct Step {
-  const char* name;  // profiling name; "<name>.weight" and "<name>.bias" in the state dict
-  Op op;             // kOpFirst: 3x3x3 conv from the input patches; kOpConv3Pool: 3x3x3 conv feeding a (1,2,2) max pool
-  int cin, cout;     // cout -1: the head, whose channels come from its weight tensor
-  Act a, b;          // source, and the skip connection concatenated after it (torch.cat([a, b]))
-  Act dst, pool;     // output, and its (1,2,2) max pool
-  int level;         // resolution of the sources: the patch, then (Y/2, X/2) and (Y/4, X/4)
-};
-// execution order
-const Step kNet[] = {
-    {"enc0.0", kOpFirst, 1, 16, kIn, kNoAct, kE0a, kNoAct, 0},
-    {"enc0.2", kOpConv3Pool, 16, 16, kE0a, kNoAct, kE0, kP0, 0},
-    {"enc1.0", kOpConv3, 16, 32, kP0, kNoAct, kE1a, kNoAct, 1},
-    {"enc1.2", kOpConv3Pool, 32, 32, kE1a, kNoAct, kE1, kP1, 1},
-    {"enc2.0", kOpConv3, 32, 64, kP1, kNoAct, kE2a, kNoAct, 2},
-    {"enc2.2", kOpConv3, 64, 64, kE2a, kNoAct, kE2, kNoAct, 2},
-    {"up1", kOpConvT, 64, 32, kE2, kNoAct, kU1, kNoAct, 2},
-    {"dec1.0", kOpConv3, 64, 32, kU1, kE1, kD1a, kNoAct, 1},
-    {"dec1.2", kOpConv3, 32, 32, kD1a, kNoAct, kD1, kNoAct, 1},
-    {"up0", kOpConvT, 32, 16, kD1, kNoAct, kU0, kNoAct, 1},
-    {"dec0.0", kOpConv3, 32, 16, kU0, kE0, kD0a, kNoAct, 0},
-    {"dec0.2", kOpConv3, 16, 16, kD0a, kNoAct, kD0, kNoAct, 0},
-    {"head", kOpHead, 16, -1, kD0, kNoAct, kOut, kNoAct, 0},
-};
-constexpr int kSteps = sizeof(kNet) / sizeof(kNet[0]);
-const char* const kPoolName[] = {"pool0", "pool1"};  // by level
+int Network::taps(Op op) { return op == kOpConvT ? 4 : op == kOpHead ? 1 : 27; }
 
-int taps(Op op) { return op == kOpConvT ? 4 : op == kOpHead ? 1 : 27; }
+// enc0 .. enc{d-1} down, with a (1,2,2) max pool after every level but the last; up{k} + dec{k} from level d-2 up to 0,
+// each decoder concatenating its transposed convolution with the encoder output of the same level; the 1x1x1 head.
+std::vector<Network::Step> Network::make_steps(int depth, int& acts) {
+  std::vector<Step> s;
+  acts = 2;  // kIn, kOut
+  auto act = [&] { return acts++; };
+  std::vector<Act> enc(depth), pooled(depth, kNoAct);
+  for (int k = 0; k < depth; ++k) {
+    const int w = 16 << k, last = k == depth - 1;
+    const Act mid = act();
+    if (k == 0) s.push_back({"enc0.0", kOpFirst, 1, w, kIn, kNoAct, mid, kNoAct, 0});
+    else s.push_back({"enc" + std::to_string(k) + ".0", kOpConv3, w / 2, w, pooled[k - 1], kNoAct, mid, kNoAct, k});
+    enc[k] = act();
+    if (!last) pooled[k] = act();
+    s.push_back({"enc" + std::to_string(k) + ".2", last ? kOpConv3 : kOpConv3Pool, w, w, mid, kNoAct, enc[k], pooled[k], k});
+  }
+  Act below = enc[depth - 1];
+  for (int k = depth - 2; k >= 0; --k) {
+    const int w = 16 << k;
+    const Act up = act(), mid = act(), dec = act();
+    s.push_back({"up" + std::to_string(k), kOpConvT, 2 * w, w, below, kNoAct, up, kNoAct, k + 1});
+    s.push_back({"dec" + std::to_string(k) + ".0", kOpConv3, 2 * w, w, up, enc[k], mid, kNoAct, k});
+    s.push_back({"dec" + std::to_string(k) + ".2", kOpConv3, w, w, mid, kNoAct, dec, kNoAct, k});
+    below = dec;
+  }
+  s.push_back({"head", kOpHead, 16, -1, below, kNoAct, kOut, kNoAct, 0});
+  return s;
+}
+
 // channels of an activation: the input patches have one, every other one those of the step that produces it
-int act_channels(Act a) {
-  for (const Step& st : kNet)
+int Network::act_channels(Act a) const {
+  for (const Step& st : steps_)
     if (st.dst == a || st.pool == a) return st.cout;
   return 1;
 }
-}  // namespace
 
 void Network::configure(int precision, Int3 patch, int batch) {
   if (precision != CFB_PRECISION_F32_SIMT && precision != CFB_PRECISION_F16X3_UMMA && precision != CFB_PRECISION_F16_UMMA &&
@@ -79,7 +79,7 @@ void Network::allocate() {
   };
   alloc(kOut, sizeof(float) * std::max(cnet_, 1), 0);
   const size_t bytes = tensor_cores() ? sizeof(__half) * parts() : sizeof(float);  // per channel and voxel
-  for (const Step& st : kNet) {
+  for (const Step& st : steps_) {
     if (st.op == kOpHead) continue;
     alloc(st.dst, bytes * st.cout, st.op == kOpConvT ? st.level - 1 : st.level);
     if (st.pool != kNoAct) alloc(st.pool, bytes * st.cout, st.level + 1);
@@ -90,8 +90,37 @@ bool Network::load(const std::map<std::string, std::vector<float>>& host_w, int 
   ready_ = false;
   for (ConvLayer& L : layers_) { cudaFree(L.w); cudaFree(L.bias); free_packed(L.packed); }
   layers_.clear();
-  for (const Step& st : kNet) {
-    const std::string wn = std::string(st.name) + ".weight", bn = std::string(st.name) + ".bias";
+  // the depth is the number of encoder levels in the state dict, and level k must be 16 << k channels wide
+  int depth = 0;
+  while (host_w.count("enc" + std::to_string(depth) + ".0.weight")) ++depth;
+  if (depth < 2 || depth > 4) {
+    err = "the U-Net depth must be 2, 3 or 4 (encoder levels enc0.0 .. enc{d-1}.0 in the state dict), found " + std::to_string(depth);
+    return false;
+  }
+  for (int k = 0, cin = 1; k < depth; cin = 16 << k, ++k) {
+    const size_t n = host_w.at("enc" + std::to_string(k) + ".0.weight").size();
+    if (n != (size_t)cin * (16 << k) * 27) {
+      err = "the U-Net widths must be 16, 32, 64, 128 (level k: 16 << k channels): enc" + std::to_string(k) + ".0.weight has " +
+            std::to_string(n) + " values, expected " + std::to_string((size_t)cin * (16 << k) * 27);
+      return false;
+    }
+  }
+  const int align = 1 << (depth - 1);
+  if (patch_.y % align || patch_.x % align) {
+    err = "the " + std::to_string(depth) + "-level U-Net pools (1,2,2) " + std::to_string(depth - 1) +
+          " times: patch y and x must be multiples of " + std::to_string(align);
+    return false;
+  }
+  int acts = 0;
+  std::vector<Step> steps = make_steps(depth, acts);
+  if (depth != depth_) {  // a different table: new activation buffers (the staged input patches stay)
+    for (size_t i = 1; i < act_.size(); ++i) act_[i].reset();
+    act_.resize(acts);
+  }
+  depth_ = depth;
+  steps_ = std::move(steps);
+  for (const Step& st : steps_) {
+    const std::string wn = st.name + ".weight", bn = st.name + ".bias";
     auto wi = host_w.find(wn), bi = host_w.find(bn);
     if (wi == host_w.end() || bi == host_w.end()) { err = "missing tensor " + (wi == host_w.end() ? wn : bn); return false; }
     const std::vector<float>& w = wi->second;
@@ -177,8 +206,8 @@ int Network::run(const Route& r, int nb, cudaStream_t s) {
   const bool tc = tensor_cores();
   const int P = fmt();  // the CUDA-core CP8 kernels take the number format
   ConvTail blend = r.blend;
-  blend.head_w = layers_[kSteps - 1].w;
-  blend.head_b = layers_[kSteps - 1].bias;
+  blend.head_w = layers_.back().w;
+  blend.head_b = layers_.back().bias;
   int launches = 0;
   auto issue = [&](const char* name, auto&& launch) {
     prof_begin(name, s);
@@ -186,34 +215,35 @@ int Network::run(const Route& r, int nb, cudaStream_t s) {
     prof_end(s);
     ++launches;
   };
-  for (int i = 0; i < kSteps; ++i) {
-    const Step& st = kNet[i];
+  for (size_t i = 0; i < steps_.size(); ++i) {
+    const Step& st = steps_[i];
     const ConvLayer& L = layers_[i];
     const Int3 sz{patch_.z, patch_.y >> st.level, patch_.x >> st.level};
     const int cb = st.b == kNoAct ? 0 : act_channels(st.b), ca = st.cin - cb;
     if (st.op == kOpFirst) {
       if (!tc && r.chunk)
         issue("extract", [&] { launch_extract_patches(r.chunk, r.in_dtype, r.chunk_size, blend.patches, nb, patch_, f32(kIn), s); });
-      issue(st.name, [&] {
+      issue(st.name.c_str(), [&] {
         if (!tc) launch_conv3_f32(f32(kIn), 1, nullptr, 0, L.w, L.bias, f32(st.dst), st.cout, nb, sz, /*relu=*/true, s);
         else if (r.chunk) launch_first_conv_cp8(r.chunk, r.in_dtype, r.chunk_size, blend.patches, nb, sz, first_w_, cp8(st.dst), P, s);
         else launch_first_conv_cp8_from_patches(f32(kIn), nb, sz, first_w_, cp8(st.dst), P, s);
       });
     } else if (st.op == kOpConv3 || st.op == kOpConv3Pool) {
       const bool pool = st.op == kOpConv3Pool, fuse_pool = tc && pool && !r.checks.no_pool_fusion;
-      const bool fuse_tail = r.end == kFusedTail && kNet[i + 1].op == kOpHead;  // + head + sigmoid + crop + mask + blend
-      issue(fuse_tail ? (std::string(st.name) + "+head+blend").c_str() : st.name, [&] {
+      const bool fuse_tail = r.end == kFusedTail && steps_[i + 1].op == kOpHead;  // + head + sigmoid + crop + mask + blend
+      issue(fuse_tail ? (st.name + "+head+blend").c_str() : st.name.c_str(), [&] {
         if (!tc) launch_conv3_f32(f32(st.a), ca, cb ? f32(st.b) : nullptr, cb, L.w, L.bias, f32(st.dst), st.cout, nb, sz, true, s);
         else launch_conv3_wgmma(cp8(st.a), ca, cb ? cp8(st.b) : nullptr, cb, L.packed, cp8(st.dst), nb, sz, /*relu=*/true, s,
                                 fuse_tail ? &blend : nullptr, fuse_pool ? cp8(st.pool) : nullptr);
       });
+      if (tc && st.cout > 64) ++launches;  // a 128-channel layer: one launch per 64-channel half (kernels_wgmma_wide.cu)
       if (pool && !fuse_pool)
-        issue(kPoolName[st.level], [&] {
+        issue(("pool" + std::to_string(st.level)).c_str(), [&] {
           if (tc) launch_maxpool_cp8(cp8(st.dst), cp8(st.pool), st.cout, P, nb, sz, s);
           else launch_maxpool_f32(f32(st.dst), f32(st.pool), st.cout, nb, sz, s);
         });
     } else if (st.op == kOpConvT) {
-      issue(st.name, [&] {
+      issue(st.name.c_str(), [&] {
         if (!tc) launch_convT_f32(f32(st.a), L.w, L.bias, f32(st.dst), st.cin, st.cout, nb, sz, s);
         else if (r.checks.simt_convt) launch_convT_cp8(cp8(st.a), L.w, L.bias, cp8(st.dst), st.cin, st.cout, P, nb, sz, s);
         else launch_convT_wgmma(cp8(st.a), L.packed, cp8(st.dst), nb, sz, s);
@@ -224,7 +254,7 @@ int Network::run(const Route& r, int nb, cudaStream_t s) {
                               nb, blend.out, blend.channels, blend.out_size, blend.scale, s);
       });
     } else if (r.end != kFusedTail) {
-      issue(st.name, [&] {
+      issue(st.name.c_str(), [&] {
         if (tc) launch_head_sigmoid_cp8(cp8(st.a), L.w, L.bias, f32(st.dst), st.cin, cnet_, P, nb, sz, s);
         else launch_head_sigmoid_f32(f32(st.a), L.w, L.bias, f32(st.dst), st.cin, cnet_, nb, sz, s);
       });

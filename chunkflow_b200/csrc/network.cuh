@@ -1,8 +1,8 @@
-// The fixed 3-level 3D U-Net (chunkflow_b200/convnet/unet3l.py) on the device.
-// Owns the packed weights and the activation workspace for `batch` patches in flight and
-// dispatches each layer to the kernels of the configured precision mode.
+// The plain 3D U-Net family of chunkflow_b200/convnet/unet3l.py (depth 2, 3 or 4, widths 16, 32, ..., (1,2,2) pooling) on
+// the device.  The layer table is generated from the depth and widths found in the state dict; the network owns the packed
+// weights and the activation workspace for `batch` patches in flight and dispatches each layer to the kernels of the
+// configured precision mode.
 #pragma once
-#include <array>
 #include <map>
 #include <string>
 #include <vector>
@@ -13,8 +13,9 @@
 
 namespace cfb {
 
-// The activations of the network; the layer table in network.cu says which step produces each one.
-enum Act : int { kIn, kE0a, kE0, kP0, kE1a, kE1, kP1, kE2a, kE2, kU1, kD1a, kD1, kU0, kD0a, kD0, kOut, kNumActs, kNoAct = -1 };
+// Activations are numbered by the layer table (network.cu); the input patches and the raw output come first.
+using Act = int;
+constexpr Act kIn = 0, kOut = 1, kNoAct = -1;
 
 struct ConvLayer {
   float* w = nullptr;     // fp32, state_dict layout
@@ -68,6 +69,19 @@ class Network {
   // Issues every step of the layer table for `nb` patches with the kernels of the configured mode; returns the launches.
   int run(const Route& r, int nb, cudaStream_t s);
 
+  enum Op { kOpFirst, kOpConv3, kOpConv3Pool, kOpConvT, kOpHead };
+  struct Step {
+    std::string name;  // profiling name; "<name>.weight" and "<name>.bias" in the state dict
+    Op op;             // kOpFirst: 3x3x3 conv from the input patches; kOpConv3Pool: 3x3x3 conv feeding a (1,2,2) max pool
+    int cin, cout;     // cout -1: the head, whose channels come from its weight tensor
+    Act a, b;          // source, and the skip connection concatenated after it (torch.cat([a, b]))
+    Act dst, pool;     // output, and its (1,2,2) max pool
+    int level;         // resolution of the sources: (Y, X) >> level
+  };
+  // The layer table of the U-Net of this depth and widths (16 << level), in execution order; `acts` gets the activation count.
+  static std::vector<Step> make_steps(int depth, int& acts);
+  static int taps(Op op);
+  int act_channels(Act a) const;
   void allocate();
   bool tensor_cores() const { return precision_ != CFB_PRECISION_F32_SIMT; }
   // activation number format of the tensor-core path (act_format.cuh) and its planes per 8-channel chunk
@@ -95,9 +109,11 @@ class Network {
   bool ready_ = false;
   int cnet_ = 0;
   FirstConvW first_w_{};              // host copy of the first layer, passed to its kernel by value
+  int depth_ = 0;                     // levels of the committed network, 0 before the first commit
+  std::vector<Step> steps_;           // the layer table of the committed network
   std::vector<ConvLayer> layers_;     // by index into the layer table
   // (batch, C, Z, Y, X) fp32 for kIn, kOut and every activation of the simt mode, CP8 for the tensor-core modes
-  std::array<DeviceBuffer, kNumActs> act_;
+  std::vector<DeviceBuffer> act_ = std::vector<DeviceBuffer>(2);
 };
 
 }  // namespace cfb

@@ -7,7 +7,7 @@ chunk is uploaded once, every patch is extracted, run through the network, bump-
 and blended by CUDA kernels on the device, and the normalised result is downloaded once.
 
 Frameworks:
-  'b200'      the fixed 3-level U-Net (chunkflow_b200/convnet/unet3l.py) as sm_90a kernels.
+  'b200'      the plain U-Net family of depth 2 to 4 (chunkflow_b200/convnet/unet3l.py) as sm_90a kernels.
   'pytorch'   accepted when the model file is that canonical U-Net (the same file drives the
               reference's ``-f pytorch`` CPU path, the parity oracle); any other torch model
               is refused -- there is no CPU / eager fallback.
@@ -158,8 +158,9 @@ class Inferencer(object):
     def _patches_in_flight(self, framework_code) -> int:
         """``batch_size`` is a scheduling hint here (the reference asserts 1 for pytorch although its examples pass
         12, inferencer.py:216-220).  With the default of 1 the device network path picks the number of patches in
-        flight itself: enough CTAs to fill 132 SMs at every U-Net level, bounded by a quarter of the free memory
-        (about 540 bytes of fp16 hi/lo activations per patch voxel)."""
+        flight itself: enough CTAs to fill 132 SMs at every U-Net level, bounded by a quarter of the free memory at
+        600 bytes per patch voxel: the activations of the default f16f8 mode take about 552 bytes per patch voxel at
+        depth 3 and about 620 at depth 4 (the 4-level network may hold a few percent more than the quarter)."""
         if self.batch_size > 1 or framework_code != _native.FRAMEWORK_UNET3L:
             return self.batch_size
         free, _ = _native.device_memory(self.device)
@@ -170,7 +171,7 @@ class Inferencer(object):
         self.patch_inferencer = None   # host-side per-patch plugin (universal / prebuilt) if any
         if framework == 'pytorch' and not b200_patch.is_canonical_model(convnet_model):
             raise NotImplementedError(
-                "framework='pytorch' is served by hand-written kernels for the canonical 3-level U-Net "
+                "framework='pytorch' is served by hand-written kernels for the plain U-Net family of depth 2 to 4 "
                 "(chunkflow_b200/convnet/unet3l.py) only; arbitrary torch models have no CPU/eager fallback here. "
                 "Wrap other backends as a `universal` plugin.")
         if framework in ('b200', 'pytorch'):

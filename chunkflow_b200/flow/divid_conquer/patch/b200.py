@@ -1,6 +1,6 @@
 """Patch backends that run on the GPU through the C-ABI.
 
-``B200``     : the fixed 3-level U-Net forward + crop + bump mask on the device, with the
+``B200``     : the U-Net forward (depth 2 to 4, from the weights) + crop + bump mask on the device, with the
                per-patch numpy API of the reference's ``PyTorch`` backend
                (chunkflow/flow/divid_conquer/patch/pytorch.py:10-119).  Usable as
                ``Inferencer(framework='prebuilt', convnet_model=B200(...))`` -- also inside
@@ -26,7 +26,7 @@ DEFAULT_MODEL_FILE = os.path.normpath(DEFAULT_MODEL_FILE)
 
 
 def is_canonical_model(convnet_model) -> bool:
-    """True if the model file is (or re-exports) the 3-level U-Net the kernels implement."""
+    """True if the model file is (or re-exports) the U-Net family the kernels implement (convnet/unet3l.py)."""
     if convnet_model is None:
         return True
     try:

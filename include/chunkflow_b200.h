@@ -56,7 +56,7 @@ extern "C" {
 #define CFB_ERR_CAPACITY (-6) /* a caller-sized table is too small: call again with a larger one */
 
 /* framework: which patch backend runs on the device */
-#define CFB_FRAMEWORK_UNET3L 0   /* fixed 3-level 3D U-Net (chunkflow_b200/convnet/unet3l.py) */
+#define CFB_FRAMEWORK_UNET3L 0   /* plain 3D U-Net of depth 2-4 (chunkflow_b200/convnet/unet3l.py), depth from the weights */
 #define CFB_FRAMEWORK_IDENTITY 1 /* reference patch/identity.py: output = input patch */
 
 /* precision of the convolution stack */
