@@ -34,26 +34,23 @@ int64_t clahe_workspace_bytes(const ClaheGeom& g, int64_t z) {
   return clahe_small_tiles(g) ? 0 : clahe_batch(g, z) * g.tiles_x * g.tiles_y * kClaheBins;
 }
 
-void clahe_run(const uint8_t* in, uint8_t* out, int64_t z, const ClaheGeom& g, uint8_t* luts, cudaStream_t st) {
+void clahe_run_small(const uint8_t* in, uint8_t* out, int64_t z, const ClaheGeom& g, cudaStream_t st) {
+  const ClaheRegion reg = clahe_small_region(g);
+  const int64_t regions = ceil_div64(g.tiles_x, reg.rx) * ceil_div64(g.tiles_y, reg.ry);
+  const int smem = (int)clahe_small_smem_bytes(g, reg);
+  CFB_CUDA(cudaFuncSetAttribute(clahe_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  const dim3 grid((unsigned)std::min<int64_t>(regions, 1 << 20), (unsigned)std::min<int64_t>(z, 65535));
+  launch(clahe_small_kernel, grid, kClaheThreads, smem, st, in, out, z, g, reg);
+}
+
+// the table path in batches of `batch` sections, whose LUTs fill `luts`
+void clahe_run_table(const uint8_t* in, uint8_t* out, int64_t z, const ClaheGeom& g, uint8_t* luts, int64_t batch, cudaStream_t st) {
   const int64_t section = g.H * g.W, tiles = g.tiles_x * g.tiles_y;
-  if (clahe_small_tiles(g)) {
-    const ClaheRegion reg = clahe_small_region(g);
-    const int64_t regions = ceil_div64(g.tiles_x, reg.rx) * ceil_div64(g.tiles_y, reg.ry);
-    const int smem = (int)clahe_small_smem_bytes(g, reg);
-    CFB_CUDA(cudaFuncSetAttribute(clahe_small_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    const dim3 grid((unsigned)std::min<int64_t>(regions, 1 << 20), (unsigned)std::min<int64_t>(z, 65535));
-    clahe_small_kernel<<<grid, kClaheThreads, smem, st>>>(in, out, z, g, reg);
-    CFB_LAUNCH_CHECK();
-    return;
-  }
-  const int64_t nb_max = clahe_batch(g, z);
-  for (int64_t z0 = 0; z0 < z; z0 += nb_max) {
-    const int64_t nb = std::min(nb_max, z - z0);
+  for (int64_t z0 = 0; z0 < z; z0 += batch) {
+    const int64_t nb = std::min(batch, z - z0);
     const dim3 grid((unsigned)std::min<int64_t>(tiles, 1 << 20), (unsigned)std::min<int64_t>(nb, 65535));
-    clahe_lut_kernel<<<grid, kClaheThreads, 0, st>>>(in + z0 * section, nb, g, luts);
-    CFB_LAUNCH_CHECK();
-    clahe_table_kernel<<<grid, kClaheThreads, 0, st>>>(in + z0 * section, out + z0 * section, nb, g, luts);
-    CFB_LAUNCH_CHECK();
+    launch(clahe_lut_kernel, grid, kClaheThreads, 0, st, in + z0 * section, nb, g, luts);
+    launch(clahe_table_kernel, grid, kClaheThreads, 0, st, in + z0 * section, out + z0 * section, nb, g, luts);
   }
 }
 
@@ -85,7 +82,10 @@ extern "C" int cfb_clahe_device(const void* d_in, void* d_out, int64_t z, int64_
       if ((w < p + bytes && p < w + need) || (w < q + bytes && q < w + need))
         throw std::invalid_argument("clahe: the workspace overlaps the input or the output");
     }
-    clahe_run((const uint8_t*)d_in, (uint8_t*)d_out, z, g, (uint8_t*)d_workspace, (cudaStream_t)stream);
+    if (clahe_small_tiles(g))
+      clahe_run_small((const uint8_t*)d_in, (uint8_t*)d_out, z, g, (cudaStream_t)stream);
+    else
+      clahe_run_table((const uint8_t*)d_in, (uint8_t*)d_out, z, g, (uint8_t*)d_workspace, clahe_batch(g, z), (cudaStream_t)stream);
     return CFB_OK;
   });
 }

@@ -1,5 +1,5 @@
-// Device code of `clahe` (DESIGN.md section 0, row f9), included by clahe.cu and, behind a one-lane shim, by
-// tests/host_emulation/clahe_emulation.cpp.  The arithmetic is OpenCV's cv2.createCLAHE(clip, (tiles_x, tiles_y)).apply on
+// Device code of `clahe` (DESIGN.md section 0, row f9), included by clahe.cu (which tests/host_emulation also compiles for
+// the host, behind a one-lane CUDA shim).  The arithmetic is OpenCV's cv2.createCLAHE(clip, (tiles_x, tiles_y)).apply on
 // uint8 sections, which the reference's plugins/clahe.py runs on every z, restated in oracle/clahe_oracle.py:
 //   tiles      th x tw pixels of the section padded at the bottom and right (BORDER_REFLECT_101: flt_fold kFltMirror), the
 //              padded section never materialised: a tile reads its rows and columns through the index map;

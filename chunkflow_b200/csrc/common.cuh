@@ -34,6 +34,16 @@ struct CudaError : std::runtime_error {
 
 #define CFB_LAUNCH_CHECK() CFB_CUDA(cudaGetLastError())
 
+#ifdef __CUDACC__
+// kernel<<<grid, block, smem, stream>>>(args...), then a CudaError if the launch failed.  The host emulations under
+// tests/host_emulation compile the operators with g++ and a fake runtime header that defines its own launch.
+template <typename... P, typename... A>
+void launch(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, A&&... args) {
+  kernel<<<grid, block, smem, stream>>>(std::forward<A>(args)...);
+  CFB_LAUNCH_CHECK();
+}
+#endif
+
 // The error boundary of every C-ABI entry point: an exception becomes a status code, its message cfb_last_error().
 template <typename F>
 int guarded(F&& f) {

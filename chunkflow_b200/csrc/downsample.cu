@@ -69,21 +69,16 @@ void ds_launch_level(const DsLevel& l, int kind, const void* in, void* out, cuda
   ds_launch_geometry(l.out, grid, block);
   const T* src = static_cast<const T*>(in);
   T* dst = static_cast<T*>(out);
-  if (l.algo == kDsStride) ds_stride_kernel<T><<<grid, block, 0, s>>>(src, l.in, l.out, l.factor, dst);
+  if (l.algo == kDsStride) launch(ds_stride_kernel<T>, grid, block, 0, s, src, l.in, l.out, l.factor, dst);
   else if constexpr (sizeof(T) == 1) throw std::logic_error("downsample: a boolean volume is only strided");
-  else if (l.algo == kDsCountless3d) ds_countless3d_kernel<T><<<grid, block, 0, s>>>(src, l.in, l.out, dst);
-  else if (kind == kDsU64) ds_countless2d_kernel<T, false><<<grid, block, 0, s>>>(src, l.in, l.out, l.preserved, dst);
-  else ds_countless2d_kernel<T, true><<<grid, block, 0, s>>>(src, l.in, l.out, l.preserved, dst);   // widened: every id counts
-  CFB_LAUNCH_CHECK();
+  else if (l.algo == kDsCountless3d) launch(ds_countless3d_kernel<T>, grid, block, 0, s, src, l.in, l.out, dst);
+  else if (kind == kDsU64) launch(ds_countless2d_kernel<T, false>, grid, block, 0, s, src, l.in, l.out, l.preserved, dst);
+  else launch(ds_countless2d_kernel<T, true>, grid, block, 0, s, src, l.in, l.out, l.preserved, dst);   // widened: every id counts
 }
 
-}  // namespace
-}  // namespace cfb
-
-using namespace cfb;
-
-extern "C" int cfb_downsample_average_device(const uint8_t* d_in, int64_t z, int64_t y, int64_t x, const int64_t factor[3],
-                                             uint8_t* d_out, void* stream) {
+// cfb_downsample_average_device; *vectorised, when given, is set to whether the vectorised kernel ran
+int ds_average(const uint8_t* d_in, int64_t z, int64_t y, int64_t x, const int64_t factor[3], uint8_t* d_out, void* stream,
+               bool* vectorised) {
   return guarded([&]() -> int {
     const DsDims s = ds_dims(z, y, x), f = ds_factor(factor);
     if (f.z <= 0 || f.y <= 0 || f.x <= 0) throw std::invalid_argument("downsample: factors below one make no sense");
@@ -99,17 +94,28 @@ extern "C" int cfb_downsample_average_device(const uint8_t* d_in, int64_t z, int
       return CFB_OK;
     }
     dim3 grid, block;
-    if (ds_average_vectorised(s, f, d_in, d_out)) {
+    const bool vec = ds_average_vectorised(s, f, d_in, d_out);
+    if (vectorised) *vectorised = vec;
+    if (vec) {
       ds_launch_geometry({o.z, o.y, o.x / 8}, grid, block);
-      if (f.z == 1) ds_average_x2_kernel<1, 2><<<grid, block, 0, st>>>(d_in, s, o, d_out);
-      else ds_average_x2_kernel<2, 2><<<grid, block, 0, st>>>(d_in, s, o, d_out);
+      if (f.z == 1) launch(ds_average_x2_kernel<1, 2>, grid, block, 0, st, d_in, s, o, d_out);
+      else launch(ds_average_x2_kernel<2, 2>, grid, block, 0, st, d_in, s, o, d_out);
     } else {
       ds_launch_geometry(o, grid, block);
-      ds_average_kernel<<<grid, block, 0, st>>>(d_in, s, o, f, d_out);
+      launch(ds_average_kernel, grid, block, 0, st, d_in, s, o, f, d_out);
     }
-    CFB_LAUNCH_CHECK();
     return CFB_OK;
   });
+}
+
+}  // namespace
+}  // namespace cfb
+
+using namespace cfb;
+
+extern "C" int cfb_downsample_average_device(const uint8_t* d_in, int64_t z, int64_t y, int64_t x, const int64_t factor[3],
+                                             uint8_t* d_out, void* stream) {
+  return ds_average(d_in, z, y, x, factor, d_out, stream, nullptr);
 }
 
 extern "C" int cfb_downsample_workspace(int32_t dtype, int64_t z, int64_t y, int64_t x, const int64_t factor[3], int64_t out_zyx[3],

@@ -1,5 +1,5 @@
-// Device code of `downsample` (DESIGN.md section 0, row f7), included by downsample.cu and, behind a one-lane shim, by
-// tests/host_emulation/downsample_emulation.cpp.  The arithmetic is the reference's vendored numpy downsampler (reference
+// Device code of `downsample` (DESIGN.md section 0, row f7), included by downsample.cu (which tests/host_emulation also
+// compiles for the host, behind a one-lane CUDA shim).  The arithmetic is the reference's vendored numpy downsampler (reference
 // lib/igneous/downsample.py), restated in oracle/downsample_oracle.py:
 //   average     uint8, any factor: floor(block sum / voxels in the block), the block clipped at the far edges;
 //   countless2d one preserved axis: the other two halved, an odd side first grown by a copy of its first plane in front

@@ -52,11 +52,10 @@ EvTables ev_tables(void* d_workspace, int64_t slots) {
 template <typename TS>
 void ev_launch_pairs(const TS* seg, const void* gt, int32_t gt_dtype, int64_t n, const EvTables& t, cudaStream_t s) {
   const int grid = ev_grid(n);
-  if (gt_dtype == CFB_DTYPE_U8) ev_pairs_kernel<TS, uint8_t><<<grid, kT, 0, s>>>(seg, (const uint8_t*)gt, n, t);
-  else if (gt_dtype == CFB_DTYPE_U32) ev_pairs_kernel<TS, uint32_t><<<grid, kT, 0, s>>>(seg, (const uint32_t*)gt, n, t);
-  else if (gt_dtype == CFB_DTYPE_U64) ev_pairs_kernel<TS, uint64_t><<<grid, kT, 0, s>>>(seg, (const uint64_t*)gt, n, t);
+  if (gt_dtype == CFB_DTYPE_U8) launch(ev_pairs_kernel<TS, uint8_t>, grid, kT, 0, s, seg, (const uint8_t*)gt, n, t);
+  else if (gt_dtype == CFB_DTYPE_U32) launch(ev_pairs_kernel<TS, uint32_t>, grid, kT, 0, s, seg, (const uint32_t*)gt, n, t);
+  else if (gt_dtype == CFB_DTYPE_U64) launch(ev_pairs_kernel<TS, uint64_t>, grid, kT, 0, s, seg, (const uint64_t*)gt, n, t);
   else throw std::invalid_argument("evaluate: ground-truth dtype must be uint8, uint32 or uint64");
-  CFB_LAUNCH_CHECK();
 }
 
 }  // namespace
@@ -85,12 +84,9 @@ extern "C" int cfb_contingency_device(const void* d_seg, int32_t seg_dtype, cons
     else if (seg_dtype == CFB_DTYPE_U32) ev_launch_pairs((const uint32_t*)d_seg, d_gt, gt_dtype, n, t, s);
     else if (seg_dtype == CFB_DTYPE_U64) ev_launch_pairs((const uint64_t*)d_seg, d_gt, gt_dtype, n, t, s);
     else throw std::invalid_argument("evaluate: segmentation dtype must be uint8, uint32 or uint64");
-    ev_margins_kernel<<<ev_grid(table_slots), kT, 0, s>>>(t);
-    CFB_LAUNCH_CHECK();
-    ev_side_kernel<<<ev_grid(table_slots), kT, 0, s>>>(t.rstate, t.rall, t.rnz, table_slots, t.stats + kEvS2, t.stats + kEvXlR);
-    CFB_LAUNCH_CHECK();
-    ev_side_kernel<<<ev_grid(table_slots), kT, 0, s>>>(t.cstate, t.call, t.cnz, table_slots, t.stats + kEvS3, t.stats + kEvXlS);
-    CFB_LAUNCH_CHECK();
+    launch(ev_margins_kernel, ev_grid(table_slots), kT, 0, s, t);
+    launch(ev_side_kernel, ev_grid(table_slots), kT, 0, s, t.rstate, t.rall, t.rnz, table_slots, t.stats + kEvS2, t.stats + kEvXlR);
+    launch(ev_side_kernel, ev_grid(table_slots), kT, 0, s, t.cstate, t.call, t.cnz, table_slots, t.stats + kEvS3, t.stats + kEvXlS);
     unsigned long long h[kEvStatWords];
     CFB_CUDA(cudaMemcpyAsync(h, t.stats, sizeof(h), cudaMemcpyDeviceToHost, s));
     CFB_CUDA(cudaStreamSynchronize(s));
@@ -112,8 +108,7 @@ extern "C" int cfb_contingency_scores(void* d_workspace, int64_t table_slots, do
     cudaStream_t s = (cudaStream_t)stream;
     const EvTables t = ev_tables(d_workspace, table_slots);
     CFB_CUDA(cudaMemsetAsync(t.stats + kEvK, 0, 8, s));
-    ev_threshold_kernel<<<ev_grid(table_slots), kT, 0, s>>>(t, size_threshold);
-    CFB_LAUNCH_CHECK();
+    launch(ev_threshold_kernel, ev_grid(table_slots), kT, 0, s, t, size_threshold);
     unsigned long long h[kEvStatWords];
     CFB_CUDA(cudaMemcpyAsync(h, t.stats, sizeof(h), cudaMemcpyDeviceToHost, s));
     CFB_CUDA(cudaStreamSynchronize(s));

@@ -1,8 +1,8 @@
 // Device code of `evaluate-segmentation`: the contingency table of two label volumes and the statistics the five scores
 // need.  NOT a stand-alone header: evaluate.cu includes it inside the library's anonymous namespace (after `kT`);
-// tests/host_emulation/evaluate_emulation.cpp includes the same text behind a one-thread, one-lane CUDA shim (it defines
-// EV_WARP = 1 and the ev_* warp helpers first), so that the kernels' logic is checked against oracle/evaluation_oracle.py on
-// machines without a GPU as well.
+// tests/host_emulation/evaluate_emulation.cpp compiles evaluate.cu for the host behind a one-thread, one-lane CUDA shim
+// (EV_WARP = 1), so that the kernels and their launch sequence are checked against oracle/evaluation_oracle.py on machines
+// without a GPU as well.
 //
 // Every uint64 value is a legal label (0 and 2^64 - 1 included), so no key value can mark an empty slot: each slot carries
 // a state word (0 empty, 1 being written, 2 ready) and the keys are written by the thread that claimed the slot.

@@ -1,7 +1,7 @@
 // Host side of `evaluate-segmentation`: the five scores from the contingency-table statistics, in double and in the
 // operation order of the reference's gala code (reference chunkflow/lib/gala/evaluate.py), so that wherever the
 // reference's float64 sums are exact (n^2 < 2^53) RI, ARI, FM and the edit distance are bit-identical to it.
-// Shared by evaluate.cu and the host emulation of the kernels (tests/host_emulation/evaluate_emulation.cpp).
+// Used by evaluate.cu.
 #pragma once
 #include <cmath>
 #include <cstdint>

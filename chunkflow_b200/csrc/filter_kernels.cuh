@@ -1,6 +1,7 @@
-// Device code of `gaussian-filter` and the median filter (DESIGN.md section 0, row f8), included by filters.cu and, behind a
-// one-lane shim, by tests/host_emulation/filters_emulation.cpp.  The arithmetic is scipy.ndimage's, which the reference calls
-// (chunk/base.py:846-853, plugins/gaussian_filter.py, plugins/median_filter.py), restated in oracle/filters_oracle.py:
+// Device code of `gaussian-filter` and the median filter (DESIGN.md section 0, row f8), included by filters.cu (which
+// tests/host_emulation also compiles for the host, behind a one-lane CUDA shim).  The arithmetic is scipy.ndimage's, which
+// the reference calls (chunk/base.py:846-853, plugins/gaussian_filter.py, plugins/median_filter.py), restated in
+// oracle/filters_oracle.py:
 //   gaussian  one 1-D pass per axis with the symmetric float64 weights w[0..r] (computed by the caller with numpy):
 //             t = x[i] * w[0], then t = t + (x[i-j] + x[i+j]) * w[j] for j = r .. 1, every operation rounded on its own
 //             (__dmul_rn / __dadd_rn: nvcc would contract a * b + c into an FMA), then a cast to the element type (uint8:

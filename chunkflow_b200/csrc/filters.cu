@@ -54,24 +54,22 @@ void flt_launch_yx(const T* src, FltPlanes sp, T* dst, FltPlanes dp, int64_t nc,
   CFB_CUDA(cudaFuncSetAttribute(flt_gaussian_yx_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const dim3 grid((unsigned)std::min<int64_t>(ceil_div64(X, kFltTx), 65535), (unsigned)std::min<int64_t>(ceil_div64(Y, kFltTy), 65535),
                   (unsigned)std::min<int64_t>(nc * nz, 65535));
-  flt_gaussian_yx_kernel<T><<<grid, kFltThreads, smem, st>>>(src, sp, dst, dp, nc, nz, Y, X, wy, wx);
-  CFB_LAUNCH_CHECK();
+  launch(flt_gaussian_yx_kernel<T>, grid, kFltThreads, smem, st, src, sp, dst, dp, nc, nz, Y, X, wy, wx);
 }
 
+// in place, in batches of `batch` sections through `work`
 template <typename T>
 void flt_gaussian(T* data, const FltDims& d, const FltWeights& wc, bool channel_pass, const FltWeights& wy,
-                  const FltWeights& wx, T* work, cudaStream_t st) {
+                  const FltWeights& wx, T* work, int64_t batch, cudaStream_t st) {
   const int64_t C = d.n[0], Z = d.n[1], Y = d.n[2], X = d.n[3], yx = Y * X;
-  const int64_t nb_max = flt_batch(d, sizeof(T));
-  for (int64_t z0 = 0; z0 < Z; z0 += nb_max) {
-    const int64_t nb = std::min(nb_max, Z - z0);
+  for (int64_t z0 = 0; z0 < Z; z0 += batch) {
+    const int64_t nb = std::min(batch, Z - z0);
     const FltPlanes chunk{Z * yx, yx}, ws{nb * yx, yx};
     T* at = data + z0 * yx;
     if (channel_pass) {
       const dim3 grid((unsigned)std::min<int64_t>(ceil_div64(yx, kFltThreads), 4096), (unsigned)std::min<int64_t>(nb, 65535),
                       (unsigned)std::min<int64_t>(C, 65535));
-      flt_gaussian_c_kernel<T><<<grid, kFltThreads, 0, st>>>(at, chunk, work, ws, C, nb, yx, wc);
-      CFB_LAUNCH_CHECK();
+      launch(flt_gaussian_c_kernel<T>, grid, kFltThreads, 0, st, at, chunk, work, ws, C, nb, yx, wc);
       flt_launch_yx<T>(work, ws, at, chunk, C, nb, Y, X, wy, wx, st);
     } else {
       flt_launch_yx<T>(at, chunk, work, ws, C, nb, Y, X, wy, wx, st);
@@ -85,15 +83,14 @@ template <typename T>
 void flt_launch_median(const T* in, const FltDims& n, const FltDims& size, int mode, T* out, cudaStream_t st) {
   const int path = flt_median_path(size);
   if (path < 0) {
-    flt_median_z3_kernel<T><<<flt_grid_1d(n.n[0] * n.n[2] * n.n[3]), kFltThreads, 0, st>>>(in, n, mode, out);
+    launch(flt_median_z3_kernel<T>, flt_grid_1d(n.n[0] * n.n[2] * n.n[3]), kFltThreads, 0, st, in, n, mode, out);
   } else {
     const dim3 grid = flt_grid_1d(n.n[0] * n.n[1] * n.n[2] * n.n[3]);
-    if (path == 4) flt_median_kernel<T, 4><<<grid, kFltThreads, 0, st>>>(in, n, size, mode, out);
-    else if (path == 16) flt_median_kernel<T, 16><<<grid, kFltThreads, 0, st>>>(in, n, size, mode, out);
-    else if (path == 32) flt_median_kernel<T, 32><<<grid, kFltThreads, 0, st>>>(in, n, size, mode, out);
-    else flt_median_kernel<T, 0><<<grid, kFltThreads, 0, st>>>(in, n, size, mode, out);
+    if (path == 4) launch(flt_median_kernel<T, 4>, grid, kFltThreads, 0, st, in, n, size, mode, out);
+    else if (path == 16) launch(flt_median_kernel<T, 16>, grid, kFltThreads, 0, st, in, n, size, mode, out);
+    else if (path == 32) launch(flt_median_kernel<T, 32>, grid, kFltThreads, 0, st, in, n, size, mode, out);
+    else launch(flt_median_kernel<T, 0>, grid, kFltThreads, 0, st, in, n, size, mode, out);
   }
-  CFB_LAUNCH_CHECK();
 }
 
 }  // namespace
@@ -119,16 +116,16 @@ extern "C" int cfb_gaussian_filter_device(void* d_data, int32_t dtype, int64_t c
     const FltDims d = flt_dims(c, z, y, x);
     const FltWeights wc = flt_weights(w_c, r_c, "c"), wy = flt_weights(w_y, r_y, "y"), wx = flt_weights(w_x, r_x, "x");
     if (!d_data || !d_workspace) throw std::invalid_argument("gaussian filter: null argument");
-    const int64_t need = flt_batch(d, esize) * c * y * x * esize;
+    const int64_t batch = flt_batch(d, esize), need = batch * c * y * x * esize;
     if (workspace_bytes < need) throw std::invalid_argument("gaussian filter: the workspace is smaller than cfb_gaussian_filter_workspace");
     const char *p = (const char*)d_data, *q = (const char*)d_workspace;
     if (p < q + need && q < p + c * z * y * x * esize) throw std::invalid_argument("gaussian filter: chunk and workspace overlap");
     cudaStream_t st = (cudaStream_t)stream;
     if (!w_c && !w_y && !w_x) return CFB_OK;
     if (dtype == CFB_DTYPE_U8)
-      flt_gaussian<uint8_t>((uint8_t*)d_data, d, wc, w_c != nullptr, wy, wx, (uint8_t*)d_workspace, st);
+      flt_gaussian<uint8_t>((uint8_t*)d_data, d, wc, w_c != nullptr, wy, wx, (uint8_t*)d_workspace, batch, st);
     else
-      flt_gaussian<float>((float*)d_data, d, wc, w_c != nullptr, wy, wx, (float*)d_workspace, st);
+      flt_gaussian<float>((float*)d_data, d, wc, w_c != nullptr, wy, wx, (float*)d_workspace, batch, st);
     return CFB_OK;
   });
 }

@@ -1,5 +1,5 @@
 // One index map per boundary mode, shared by the smoothing filters (filter_kernels.cuh, DESIGN.md section 0, row f8) and
-// `clahe` (clahe_kernels.cuh, row f9).  Included inside the anonymous namespace of each .cu file and by the host emulations.
+// `clahe` (clahe_kernels.cuh, row f9).  Included inside the anonymous namespace of each .cu file.
 #pragma once
 
 enum FltMode { kFltReflect = 0, kFltNearest = 1, kFltMirror = 2, kFltWrap = 3, kFltConstant = 4 };

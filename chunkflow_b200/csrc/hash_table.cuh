@@ -1,8 +1,7 @@
 // Open-addressing hash tables in global memory, shared by the region graph (watershed_kernels.cuh) and the contingency
 // table (evaluate_kernels.cuh).  Linear probing from rg_hash(key) & mask; a key that finds no place within kRgMaxProbe
 // slots raises the table's overflow flag and the host retries with a larger table (CFB_ERR_CAPACITY).
-// NOT a stand-alone header: included inside the library's anonymous namespace, and by the host emulations behind their
-// one-thread CUDA shims.
+// NOT a stand-alone header: included inside the library's anonymous namespace.
 #pragma once
 
 constexpr int kRgMaxProbe = 1024;

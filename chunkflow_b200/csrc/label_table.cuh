@@ -1,7 +1,8 @@
 // Device code of the segmentation clean-up (`mask-out-objects`, `remap-segmentation`, DeviceChunk.unique): the table of a
 // label volume and the relabelling it plans.  NOT a stand-alone header: relabel.cu includes it inside the library's anonymous
-// namespace (after `kT`); tests/host_emulation/relabel_emulation.cpp includes the same text behind a one-thread, one-lane CUDA
-// shim (EV_WARP = 1), so that the kernels' logic is checked against oracle/relabel_oracle.py on machines without a GPU.
+// namespace (after `kT`); tests/host_emulation/relabel_emulation.cpp compiles relabel.cu for the host behind a one-thread,
+// one-lane CUDA shim (EV_WARP = 1), so that the kernels and their launch sequences are checked against oracle/relabel_oracle.py
+// on machines without a GPU.
 //
 // One table (state_table.cuh: any uint64 is a legal id), a power of two of slots:
 //   id -> (voxel count, linear index of the id's first voxel in raster order, new value)

@@ -60,9 +60,8 @@ LtTable lt_table(void* d_workspace, int64_t slots) {
 template <typename TI>
 void lt_launch_apply(const TI* in, int64_t n, const LtTable& t, void* out, int32_t out_dtype, cudaStream_t s) {
   const int grid = lt_grid(ceil_div64(n, 16 / (int64_t)sizeof(TI)));
-  if (out_dtype == CFB_DTYPE_U64) lt_apply_kernel<TI, uint64_t><<<grid, kT, 0, s>>>(in, n, t, (uint64_t*)out);
-  else lt_apply_kernel<TI, TI><<<grid, kT, 0, s>>>(in, n, t, (TI*)out);
-  CFB_LAUNCH_CHECK();
+  if (out_dtype == CFB_DTYPE_U64) launch(lt_apply_kernel<TI, uint64_t>, grid, kT, 0, s, in, n, t, (uint64_t*)out);
+  else launch(lt_apply_kernel<TI, TI>, grid, kT, 0, s, in, n, t, (TI*)out);
 }
 
 }  // namespace
@@ -91,10 +90,9 @@ extern "C" int cfb_label_table_device(const void* d_labels, int32_t dtype, int64
     CFB_CUDA(cudaMemsetAsync(t.state, 0, (size_t)table_slots * 2 * 4, s));      // states and counts
     CFB_CUDA(cudaMemsetAsync(t.first, 0xFF, (size_t)table_slots * 4, s));       // atomicMin target
     const int grid = lt_grid(ceil_div64(n, 16 / lt_dtype_bytes(dtype)));
-    if (dtype == CFB_DTYPE_U8) lt_count_kernel<uint8_t><<<grid, kT, 0, s>>>((const uint8_t*)d_labels, n, t);
-    else if (dtype == CFB_DTYPE_U32) lt_count_kernel<uint32_t><<<grid, kT, 0, s>>>((const uint32_t*)d_labels, n, t);
-    else lt_count_kernel<uint64_t><<<grid, kT, 0, s>>>((const uint64_t*)d_labels, n, t);
-    CFB_LAUNCH_CHECK();
+    if (dtype == CFB_DTYPE_U8) launch(lt_count_kernel<uint8_t>, grid, kT, 0, s, (const uint8_t*)d_labels, n, t);
+    else if (dtype == CFB_DTYPE_U32) launch(lt_count_kernel<uint32_t>, grid, kT, 0, s, (const uint32_t*)d_labels, n, t);
+    else launch(lt_count_kernel<uint64_t>, grid, kT, 0, s, (const uint64_t*)d_labels, n, t);
     unsigned long long h[kLtStatWords];
     CFB_CUDA(cudaMemcpyAsync(h, t.stats, sizeof(h), cudaMemcpyDeviceToHost, s));
     CFB_CUDA(cudaStreamSynchronize(s));
@@ -159,20 +157,13 @@ extern "C" int cfb_label_table_plan(void* d_workspace, int64_t table_slots, int6
     CFB_CUDA(cudaMemsetAsync(t.stats + kLtDust, 0, (kLtStatWords - kLtDust) * 8, s));
     CFB_CUDA(cudaMemsetAsync(t.flags, 0, (size_t)table_slots * 4, s));
     if (renumber) CFB_CUDA(cudaMemsetAsync(bits, 0, (size_t)nblocks * kLtBlockWords * 4, s));
-    if (num_keep > 0) {
-      lt_keep_kernel<<<lt_grid(num_keep), kT, 0, s>>>((const unsigned long long*)d_keep_ids, num_keep, t);
-      CFB_LAUNCH_CHECK();
-    }
-    lt_decide_kernel<<<lt_grid(table_slots), kT, 0, s>>>(t, use_dust ? 1 : 0, (long long)dust_threshold, use_keep ? 1 : 0,
-                                                         renumber ? 1 : 0, bits);
-    CFB_LAUNCH_CHECK();
+    if (num_keep > 0) launch(lt_keep_kernel, lt_grid(num_keep), kT, 0, s, (const unsigned long long*)d_keep_ids, num_keep, t);
+    launch(lt_decide_kernel, lt_grid(table_slots), kT, 0, s, t, use_dust ? 1 : 0, (long long)dust_threshold, use_keep ? 1 : 0,
+           renumber ? 1 : 0, bits);
     if (renumber) {
-      lt_block_count_kernel<<<lt_grid(nblocks * EV_WARP), kT, 0, s>>>(bits, nblocks, block_count);
-      CFB_LAUNCH_CHECK();
-      cc_scan_blocks_kernel<<<1, 1024, 0, s>>>(block_count, nblocks, d_total);
-      CFB_LAUNCH_CHECK();
-      lt_rank_kernel<<<lt_grid(table_slots), kT, 0, s>>>(t, bits, block_count, (unsigned long long)base_id);
-      CFB_LAUNCH_CHECK();
+      launch(lt_block_count_kernel, lt_grid(nblocks * EV_WARP), kT, 0, s, bits, nblocks, block_count);
+      launch(cc_scan_blocks_kernel, 1, 1024, 0, s, block_count, nblocks, d_total);
+      launch(lt_rank_kernel, lt_grid(table_slots), kT, 0, s, t, bits, block_count, (unsigned long long)base_id);
     }
     uint32_t total = 0;
     CFB_CUDA(cudaMemcpyAsync(h, t.stats, sizeof(h), cudaMemcpyDeviceToHost, s));

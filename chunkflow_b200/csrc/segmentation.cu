@@ -166,21 +166,15 @@ extern "C" int cfb_connected_components_device(const void* d_in, int32_t in_dtyp
     const int64_t nblocks = ceil_div64(n, kScanBlock);
     uint32_t* block_count = rank + n;
     uint32_t* d_num = block_count + nblocks;
-    if (in_dtype == CFB_DTYPE_U8) cc_init_kernel<uint8_t><<<grid_for(n), kT, 0, s>>>((const uint8_t*)d_in, P, val, n, 0.f);
-    else if (in_dtype == CFB_DTYPE_U32) cc_init_kernel<uint32_t><<<grid_for(n), kT, 0, s>>>((const uint32_t*)d_in, P, val, n, 0.f);
-    else if (in_dtype == CFB_DTYPE_F32) cc_init_kernel<float><<<grid_for(n), kT, 0, s>>>((const float*)d_in, P, val, n, threshold);
+    if (in_dtype == CFB_DTYPE_U8) launch(cc_init_kernel<uint8_t>, grid_for(n), kT, 0, s, (const uint8_t*)d_in, P, val, n, 0.f);
+    else if (in_dtype == CFB_DTYPE_U32) launch(cc_init_kernel<uint32_t>, grid_for(n), kT, 0, s, (const uint32_t*)d_in, P, val, n, 0.f);
+    else if (in_dtype == CFB_DTYPE_F32) launch(cc_init_kernel<float>, grid_for(n), kT, 0, s, (const float*)d_in, P, val, n, threshold);
     else throw std::invalid_argument("connected components: input dtype must be uint8, uint32 or float32 (with a threshold)");
-    CFB_LAUNCH_CHECK();
-    cc_merge_kernel<<<grid_for(n), kT, 0, s>>>(val, P, sz, nnb);
-    CFB_LAUNCH_CHECK();
-    cc_flatten_count_kernel<<<(unsigned)nblocks, kT, 0, s>>>(val, P, n, block_count);
-    CFB_LAUNCH_CHECK();
-    cc_scan_blocks_kernel<<<1, 1024, 0, s>>>(block_count, nblocks, d_num);
-    CFB_LAUNCH_CHECK();
-    cc_rank_kernel<<<(unsigned)nblocks, kT, 0, s>>>(val, P, n, block_count, rank);
-    CFB_LAUNCH_CHECK();
-    cc_relabel_kernel<<<grid_for(n), kT, 0, s>>>(val, P, rank, d_labels, n);
-    CFB_LAUNCH_CHECK();
+    launch(cc_merge_kernel, grid_for(n), kT, 0, s, val, P, sz, nnb);
+    launch(cc_flatten_count_kernel, (unsigned)nblocks, kT, 0, s, val, P, n, block_count);
+    launch(cc_scan_blocks_kernel, 1, 1024, 0, s, block_count, nblocks, d_num);
+    launch(cc_rank_kernel, (unsigned)nblocks, kT, 0, s, val, P, n, block_count, rank);
+    launch(cc_relabel_kernel, grid_for(n), kT, 0, s, val, P, rank, d_labels, n);
     if (num_labels) {
       CFB_CUDA(cudaMemcpyAsync(num_labels, d_num, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
       CFB_CUDA(cudaStreamSynchronize(s));
@@ -220,18 +214,15 @@ extern "C" int cfb_watershed_device(const float* d_affs, int32_t flip_channel, i
     uint32_t* dist = d_num + 1;
     uint32_t* d_changed = dist + n;
     const int grid = grid_for(n);
-    ws_bits_kernel<<<grid, kT, 0, s>>>(d_affs, g, flip_channel ? 1 : 0, aff_threshold_low, aff_threshold_high, P, val);
-    CFB_LAUNCH_CHECK();
-    ws_corner_kernel<<<grid, kT, 0, s>>>(val, g, dist);
-    CFB_LAUNCH_CHECK();
+    launch(ws_bits_kernel, grid, kT, 0, s, d_affs, g, flip_channel ? 1 : 0, aff_threshold_low, aff_threshold_high, P, val);
+    launch(ws_corner_kernel, grid, kT, 0, s, val, g, dist);
     // breadth-first levels in batches of 8 launches per look at the flag (a level without news ends the search; the
     // remaining launches of its batch find nothing)
     uint32_t level = 1;
     for (;;) {
       CFB_CUDA(cudaMemsetAsync(d_changed, 0, sizeof(uint32_t), s));
       for (int k = 0; k < 8; ++k, ++level) {
-        ws_bfs_kernel<<<grid, kT, 0, s>>>(val, g, dist, level, d_changed);
-        CFB_LAUNCH_CHECK();
+        launch(ws_bfs_kernel, grid, kT, 0, s, val, g, dist, level, d_changed);
       }
       uint32_t changed = 0;
       CFB_CUDA(cudaMemcpyAsync(&changed, d_changed, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
@@ -239,16 +230,11 @@ extern "C" int cfb_watershed_device(const float* d_affs, int32_t flip_channel, i
       if (!changed) break;
       if (level > 0x7FFFFFF0u) throw std::runtime_error("watershed: plateau search did not end");
     }
-    ws_merge_kernel<<<grid, kT, 0, s>>>(val, dist, g, P);
-    CFB_LAUNCH_CHECK();
-    cc_flatten_count_kernel<<<(unsigned)nblocks, kT, 0, s>>>(val, P, n, block_count);
-    CFB_LAUNCH_CHECK();
-    cc_scan_blocks_kernel<<<1, 1024, 0, s>>>(block_count, nblocks, d_num);
-    CFB_LAUNCH_CHECK();
-    cc_rank_kernel<<<(unsigned)nblocks, kT, 0, s>>>(val, P, n, block_count, rank);
-    CFB_LAUNCH_CHECK();
-    cc_relabel_kernel<<<grid, kT, 0, s>>>(val, P, rank, d_fragments, n);
-    CFB_LAUNCH_CHECK();
+    launch(ws_merge_kernel, grid, kT, 0, s, val, dist, g, P);
+    launch(cc_flatten_count_kernel, (unsigned)nblocks, kT, 0, s, val, P, n, block_count);
+    launch(cc_scan_blocks_kernel, 1, 1024, 0, s, block_count, nblocks, d_num);
+    launch(cc_rank_kernel, (unsigned)nblocks, kT, 0, s, val, P, n, block_count, rank);
+    launch(cc_relabel_kernel, grid, kT, 0, s, val, P, rank, d_fragments, n);
     if (num_fragments) {
       CFB_CUDA(cudaMemcpyAsync(num_fragments, d_num, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
       CFB_CUDA(cudaStreamSynchronize(s));
@@ -279,9 +265,8 @@ extern "C" int cfb_region_graph_device(const float* d_affs, int32_t flip_channel
     CFB_CUDA(cudaMemsetAsync(keys, 0, (size_t)table_slots * 16, s));     // keys + sums
     CFB_CUDA(cudaMemsetAsync(counts, 0, (size_t)table_slots * 4, s));
     CFB_CUDA(cudaMemsetAsync(info, 0, 4 * sizeof(uint32_t), s));
-    rg_accumulate_kernel<<<grid_for(g.n), kT, 0, s>>>(d_affs, d_fragments, g, flip_channel ? 1 : 0, keys, sums, counts,
-                                                     (unsigned long long)(table_slots - 1), info);
-    CFB_LAUNCH_CHECK();
+    launch(rg_accumulate_kernel, grid_for(g.n), kT, 0, s, d_affs, d_fragments, g, flip_channel ? 1 : 0, keys, sums, counts,
+           (unsigned long long)(table_slots - 1), info);
     uint32_t h_info[2] = {0, 0};
     CFB_CUDA(cudaMemcpyAsync(h_info, info, sizeof(h_info), cudaMemcpyDeviceToHost, s));
     CFB_CUDA(cudaStreamSynchronize(s));
@@ -309,8 +294,7 @@ extern "C" int cfb_region_graph_read(void* d_workspace, int64_t table_slots, int
     uint32_t* ocounts = counts + table_slots;
     uint32_t* cursor = ocounts + table_slots + 2;   // info[2]
     CFB_CUDA(cudaMemsetAsync(cursor, 0, sizeof(uint32_t), s));
-    rg_gather_kernel<<<grid_for(table_slots), kT, 0, s>>>(keys, sums, counts, table_slots, okeys, osums, ocounts, cursor);
-    CFB_LAUNCH_CHECK();
+    launch(rg_gather_kernel, grid_for(table_slots), kT, 0, s, keys, sums, counts, table_slots, okeys, osums, ocounts, cursor);
     std::vector<unsigned long long> k((size_t)num_edges), sm((size_t)num_edges);
     std::vector<uint32_t> ct((size_t)num_edges);
     uint32_t got = 0;
@@ -338,8 +322,7 @@ extern "C" int cfb_relabel_device(const uint32_t* d_labels, int64_t n, const uin
   return guarded([&]() -> int {
     if (!d_labels || !d_map || !d_out || n < 0 || map_size < 0 || map_size > (int64_t)UINT32_MAX) throw std::invalid_argument("relabel: bad argument");
     if (n == 0) return CFB_OK;
-    relabel_map_kernel<<<grid_for(n), kT, 0, (cudaStream_t)stream>>>(d_labels, n, d_map, (uint32_t)map_size, d_out);
-    CFB_LAUNCH_CHECK();
+    launch(relabel_map_kernel, grid_for(n), kT, 0, (cudaStream_t)stream, d_labels, n, d_map, (uint32_t)map_size, d_out);
     return CFB_OK;
   });
 }

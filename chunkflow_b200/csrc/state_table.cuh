@@ -2,8 +2,8 @@
 // (evaluate_kernels.cuh) and the label table (label_table.cuh).  No key value can mark an empty slot, so each slot carries a
 // state word (0 empty, 1 being written, 2 ready) and the keys are written by the thread that claimed the slot.  Also the
 // warp helpers both use to combine runs of equal keys before the atomics.
-// NOT a stand-alone header: included inside the library's anonymous namespace; the host emulations define EV_WARP = 1 and
-// the ev_* helpers for a one-lane warp before they include it.
+// NOT a stand-alone header: included inside the library's anonymous namespace; the CUDA shim of the host emulations
+// (tests/host_emulation/cuda_shim) defines EV_WARP = 1 and the ev_* helpers for a one-lane warp first.
 #pragma once
 
 #include "hash_table.cuh"

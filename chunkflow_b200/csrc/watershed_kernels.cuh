@@ -1,7 +1,7 @@
 // Device code of the `agglomerate` operator's voxel passes and the union-find helpers they share with connected components.
 // NOT a stand-alone header: segmentation.cu includes it inside the library's anonymous namespace (after `Int3` and `kT`);
-// tests/host_emulation/ws_emulation.cpp includes the same text behind a one-thread CUDA shim, so that the kernels' logic is
-// checked against oracle/agglomeration_oracle.py on machines without a GPU as well.
+// tests/host_emulation/ws_emulation.cpp compiles segmentation.cu for the host behind a one-thread CUDA shim, so that the
+// kernels and their launch sequences are checked against oracle/agglomeration_oracle.py on machines without a GPU as well.
 #pragma once
 
 __device__ __forceinline__ uint32_t uf_find(const uint32_t* P, uint32_t x) {

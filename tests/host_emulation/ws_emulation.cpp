@@ -1,80 +1,46 @@
-// TEST INFRASTRUCTURE: runs the device code of chunkflow_b200/csrc/watershed_kernels.cuh on the host, one "thread" (grid 1 x 1,
-// so every grid-stride loop walks the whole volume; atomics are plain read-modify-writes), so that the LOGIC of the
-// watershed / region-graph / relabel kernels is compared with oracle/agglomeration_oracle.py on machines without a GPU
-// (tests/test_segmentation_agglomerate.py builds this file with g++).  Concurrency is what the `-m gpu` tests add.
-#include <algorithm>
-#include <cmath>
-#include <cstdint>
-#include <cstring>
-#include <vector>
+// segmentation.cu on the host (tests/test_segmentation_agglomerate.py), behind the one-lane CUDA shim of
+// cuda_shim/cuda_runtime.h.  The ranking of the union-find roots in raster order is three kernels whose threads cooperate
+// through shared memory; launching one of them runs what it computes serially instead (defined below the library).
+#include <string>
 
-#define __global__
-#define __device__
-#define __forceinline__ inline
-#define __launch_bounds__(...)
-struct EmuDim { unsigned x = 0; };
-static EmuDim blockIdx, threadIdx;
-static struct { unsigned x = 1; } blockDim, gridDim;
-template <typename T> static T atomicCAS(T* p, T cmp, T v) { T o = *p; if (o == cmp) *p = v; return o; }
-template <typename T> static T atomicAdd(T* p, T v) { T o = *p; *p = o + v; return o; }
-template <typename T> static T atomicMin(T* p, T v) { T o = *p; if (v < o) *p = v; return o; }
-static long long __double2ll_rn(double v) { return std::llrint(v); }
-using std::max;
-using std::min;
+#include "scan_blocks.h"
 
-struct Int3 { int z, y, x; };
-constexpr int kT = 256;
-#include "../../chunkflow_b200/csrc/watershed_kernels.cuh"
-#include "../../chunkflow_b200/csrc/edge_sort.h"
+template <typename... A>
+void launch(void (*kernel)(const uint32_t*, uint32_t*, int64_t, uint32_t*), dim3, dim3, size_t, cudaStream_t, A&&... args);
+template <typename... A>
+void launch(void (*kernel)(const uint32_t*, const uint32_t*, int64_t, const uint32_t*, uint32_t*), dim3, dim3, size_t, cudaStream_t,
+            A&&... args);
 
-static WsGeom geom(int64_t z, int64_t y, int64_t x) {
-  WsGeom g;
-  g.sz = Int3{(int)z, (int)y, (int)x};
-  g.n = z * y * x;
-  g.step[0] = y * x; g.step[1] = x; g.step[2] = 1;
-  return g;
+#include "../../chunkflow_b200/csrc/segmentation.cu"
+
+namespace cfb {
+static std::string last_error;
+void set_last_error(const std::string& msg) { last_error = msg; }
+}  // namespace cfb
+extern "C" const char* cfb_last_error(void) { return cfb::last_error.c_str(); }
+
+// cc_flatten_count_kernel: every foreground voxel pointed at its root, the roots of every scan block counted
+template <typename... A>
+void launch(void (*kernel)(const uint32_t*, uint32_t*, int64_t, uint32_t*), dim3, dim3, size_t, cudaStream_t, A&&... args) {
+  if (kernel != cc_flatten_count_kernel) return kernel(args...);
+  [](const uint32_t* val, uint32_t* P, int64_t n, uint32_t* block_count) {
+    for (int64_t i = 0; i < n; ++i) {
+      if (i % kScanBlock == 0) block_count[i / kScanBlock] = 0;
+      if (val[i] && (P[i] = uf_find(P, (uint32_t)i)) == (uint32_t)i) ++block_count[i / kScanBlock];
+    }
+  }(args...);
 }
 
-extern "C" int emu_watershed(const float* affs, int flip, int64_t z, int64_t y, int64_t x, float low, float high, uint32_t* fragments) {
-  const WsGeom g = geom(z, y, x);
-  std::vector<uint32_t> P(g.n), val(g.n), dist(g.n);
-  ws_bits_kernel(affs, g, flip, low, high, P.data(), val.data());
-  ws_corner_kernel(val.data(), g, dist.data());
-  for (uint32_t level = 1;; ++level) {
-    uint32_t changed = 0;
-    ws_bfs_kernel(val.data(), g, dist.data(), level, &changed);
-    if (!changed) break;
-  }
-  ws_merge_kernel(val.data(), dist.data(), g, P.data());
-  // what cc_flatten_count / cc_rank / cc_relabel do on the device: roots ranked in raster order
-  std::vector<uint32_t> rank(g.n, 0);
-  uint32_t next = 0;
-  for (int64_t i = 0; i < g.n; ++i)
-    if (val[i] && uf_find(P.data(), (uint32_t)i) == (uint32_t)i) rank[i] = ++next;
-  for (int64_t i = 0; i < g.n; ++i) fragments[i] = val[i] ? rank[uf_find(P.data(), (uint32_t)i)] : 0u;
-  return (int)next;
-}
-
-// -> number of edges (sorted by key into the output arrays, capacity `slots`), -1 when the table overflowed
-extern "C" int64_t emu_region_graph(const float* affs, int flip, const uint32_t* fragments, int64_t z, int64_t y, int64_t x, int64_t slots,
-                                    uint32_t* u, uint32_t* v, uint64_t* sum_fixed, uint32_t* count) {
-  const WsGeom g = geom(z, y, x);
-  std::vector<unsigned long long> keys(slots, 0), sums(slots, 0), okeys(slots), osums(slots);
-  std::vector<uint32_t> counts(slots, 0), ocounts(slots);
-  uint32_t info[4] = {0, 0, 0, 0};
-  rg_accumulate_kernel(affs, fragments, g, flip, keys.data(), sums.data(), counts.data(), (unsigned long long)(slots - 1), info);
-  if (info[1]) return -1;
-  rg_gather_kernel(keys.data(), sums.data(), counts.data(), slots, okeys.data(), osums.data(), ocounts.data(), &info[2]);
-  if (info[2] != info[0]) return -2;
-  std::vector<uint32_t> order;
-  sorted_edge_order(okeys.data(), info[0], order);   // the product's host helper (csrc/edge_sort.h)
-  for (uint32_t i = 0; i < info[0]; ++i) {
-    const uint32_t o = order[i];
-    u[i] = (uint32_t)(okeys[o] >> 32); v[i] = (uint32_t)(okeys[o] & 0xFFFFFFFFULL); sum_fixed[i] = osums[o]; count[i] = ocounts[o];
-  }
-  return info[0];
-}
-
-extern "C" void emu_relabel(const uint32_t* labels, int64_t n, const uint32_t* map, uint32_t map_size, uint32_t* out) {
-  relabel_map_kernel(labels, n, map, map_size, out);
+// cc_rank_kernel: the rank of every root, its block's base plus the roots before it in the block
+template <typename... A>
+void launch(void (*kernel)(const uint32_t*, const uint32_t*, int64_t, const uint32_t*, uint32_t*), dim3, dim3, size_t, cudaStream_t,
+            A&&... args) {
+  if (kernel != cc_rank_kernel) return kernel(args...);
+  [](const uint32_t* val, const uint32_t* P, int64_t n, const uint32_t* block_base, uint32_t* rank) {
+    uint32_t next = 0;
+    for (int64_t i = 0; i < n; ++i) {
+      if (i % kScanBlock == 0) next = block_base[i / kScanBlock];
+      if (val[i] && P[i] == (uint32_t)i) rank[i] = next++;
+    }
+  }(args...);
 }

@@ -1,15 +1,14 @@
 """`clahe` (DESIGN.md section 0, row f9) on the CPU: the numpy oracle (oracle/clahe_oracle.py) against live OpenCV and against
 golden vectors of the reference's own plugin (tests/golden/clahe_reference.npz, made by tests/golden/make_golden_clahe.py);
-the FMA negative control; the device code of csrc/clahe_kernels.cuh, compiled for the host behind a one-lane CUDA shim
-(tests/host_emulation/clahe_emulation.cpp), against the oracle on both paths; the refusals; the command's options."""
+the FMA negative control; csrc/clahe.cu, compiled for the host behind a one-lane CUDA shim (tests/host_emulation), against
+the oracle on both paths; the refusals; the command's options."""
 import ctypes as C
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import host_emulation
 from oracle import clahe_oracle as CO
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -115,28 +114,33 @@ def test_oracle_refusals():
 # ------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if gxx is None:
-        pytest.skip("g++ not available")
-    out = tmp_path_factory.mktemp("clahe_emu") / "libclahe_emu.so"
-    src = os.path.join(ROOT, "tests", "host_emulation", "clahe_emulation.cpp")
-    subprocess.run([gxx, "-O2", "-std=c++17", "-ffp-contract=off", "-shared", "-fPIC", "-Wno-unknown-pragmas", src, "-o", str(out)],
-                   check=True)
-    lib = C.CDLL(str(out))
-    i64, vp = C.c_int64, C.c_void_p
-    lib.emu_clahe.argtypes = [vp, vp, i64, i64, i64, C.c_double, i64, i64, C.c_int, i64]
-    lib.emu_clahe.restype = C.c_int
+    lib = host_emulation.build("clahe", tmp_path_factory)
+    i32, i64, vp = C.c_int32, C.c_int64, C.c_void_p
+    lib.cfb_clahe_workspace.argtypes = [i64, i64, i64, i32, i32, C.POINTER(i64)]
+    lib.cfb_clahe_device.argtypes = [vp, vp, i64, i64, i64, C.c_double, i32, i32, vp, i64, vp]
+    lib.emu_clahe_path.argtypes = [vp, vp, i64, i64, i64, C.c_double, i32, i32, C.c_int, i64]
     lib.emu_small_region.argtypes = [i64, i64, i64, i64, vp]
     return lib
 
 
 def emu_clahe(lib, a, clip, grid, path=-1, batch=2, offset=0):
-    """-> (result, path taken); ``offset`` bytes shift the input and (by 3) the output off 16-byte alignment."""
+    """-> (result, path taken).  path -1: cfb_clahe_device with the workspace of cfb_clahe_workspace, which chooses the path
+    and the batch (the small-tile path needs none); 0 / 1: the table path in batches of ``batch`` sections / the small-tile
+    path.  ``offset`` bytes shift the input and (by 3) the output off 16-byte alignment."""
     src = np.zeros(a.size + 32, np.uint8)[offset:offset + a.size].reshape(a.shape)
     src[...] = a
     dst = np.zeros(a.size + 32, np.uint8)[3 if offset else 0:][:a.size].reshape(a.shape)
-    taken = lib.emu_clahe(C.c_void_p(src.ctypes.data), C.c_void_p(dst.ctypes.data), *a.shape, clip, grid[0], grid[1], path, batch)
-    return dst.copy(), taken
+    p = lambda b: C.c_void_p(b.ctypes.data)
+    if path < 0:
+        need = C.c_int64()
+        assert lib.cfb_clahe_workspace(*a.shape, grid[0], grid[1], C.byref(need)) == 0, lib.cfb_last_error()
+        work = np.zeros(max(need.value, 1), np.uint8)
+        rc = lib.cfb_clahe_device(p(src), p(dst), *a.shape, clip, grid[0], grid[1], p(work), need.value, None)
+        path = int(need.value == 0)
+    else:
+        rc = lib.emu_clahe_path(p(src), p(dst), *a.shape, clip, grid[0], grid[1], path, batch)
+    assert rc == 0, lib.cfb_last_error()
+    return dst.copy(), path
 
 
 def tile_pixels(y, x, grid):

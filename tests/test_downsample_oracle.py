@@ -1,18 +1,17 @@
 """`downsample` (DESIGN.md section 0, row f7; reference flow/flow.py:1545-1573, lib/igneous/downsample.py) on the CPU: the numpy
 oracle (oracle/downsample_oracle.py) against golden vectors of the REAL vendored downsampler
 (tests/golden/downsample_reference.npz, made by tests/golden/make_golden_downsample.py) and, where the reference tree exists,
-against the live module; the device code of csrc/downsample_kernels.cuh, compiled for the host behind a one-lane CUDA shim
-(tests/host_emulation/downsample_emulation.cpp), against the oracle; the command's option names; the wrappers' argument checks."""
+against the live module; csrc/downsample.cu, compiled for the host behind a one-lane CUDA shim (tests/host_emulation),
+against the oracle; the command's option names; the wrappers' argument checks."""
 import ctypes as C
 import itertools
 import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import host_emulation
 from conftest import has_gpu
 from oracle import downsample_oracle as DO
 
@@ -182,19 +181,20 @@ def test_command_dispatch():
 # ------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if gxx is None:
-        pytest.skip("g++ not available")
-    out = tmp_path_factory.mktemp("ds_emu") / "libds_emu.so"
-    src = os.path.join(ROOT, "tests", "host_emulation", "downsample_emulation.cpp")
-    subprocess.run([gxx, "-O2", "-std=c++17", "-shared", "-fPIC", "-Wno-unknown-pragmas", src, "-o", str(out)], check=True)
-    lib = C.CDLL(str(out))
-    i64 = C.c_int64
-    lib.emu_average.argtypes = [C.c_void_p, i64, i64, i64, i64, i64, i64, C.c_void_p]
-    lib.emu_average.restype = C.c_int
-    lib.emu_plan.argtypes = [C.c_int, i64, i64, i64, i64, i64, i64, C.c_void_p]
-    lib.emu_segmentation.argtypes = [C.c_int, C.c_void_p, i64, i64, i64, i64, i64, i64, C.c_void_p]
+    lib = host_emulation.build("downsample", tmp_path_factory)
+    i32, i64, vp = C.c_int32, C.c_int64, C.c_void_p
+    lib.emu_average.argtypes = [vp, i64, i64, i64, C.POINTER(i64 * 3), vp]
+    lib.emu_plan.argtypes = [C.c_int, i64, i64, i64, i64, i64, i64, vp]
+    lib.cfb_downsample_workspace.argtypes = [i32, i64, i64, i64, C.POINTER(i64 * 3), C.POINTER(i64 * 3), C.POINTER(i64)]
+    lib.cfb_downsample_segmentation_device.argtypes = [vp, i32, i64, i64, i64, C.POINTER(i64 * 3), vp, vp, vp]
     return lib
+
+
+def emu_average(lib, arr, factor, out):
+    """cfb_downsample_average_device -> 1 when it ran the vectorised kernel, 0 for the generic one."""
+    path = lib.emu_average(C.c_void_p(arr.ctypes.data), *arr.shape, C.byref((C.c_int64 * 3)(*factor)), C.c_void_p(out.ctypes.data))
+    assert path >= 0, lib.cfb_last_error()
+    return path
 
 
 def emu_run(lib, arr, factor):
@@ -203,7 +203,7 @@ def emu_run(lib, arr, factor):
     p = lambda a: C.c_void_p(a.ctypes.data)
     if arr.dtype == np.uint8:
         out = np.zeros(tuple(-(-s // f) for s, f in zip(arr.shape, factor)), np.uint8)
-        lib.emu_average(p(arr), *arr.shape, *factor, p(out))
+        emu_average(lib, arr, factor, out)
         return out
     plan = np.zeros(5 * 64, np.int64)
     n = lib.emu_plan(KINDS[arr.dtype], *arr.shape, *factor, p(plan))
@@ -212,7 +212,12 @@ def emu_run(lib, arr, factor):
     shape = tuple(plan[5 * n - 3: 5 * n]) if n else arr.shape
     out = np.zeros(shape, arr.dtype)
     src = arr.copy()
-    assert lib.emu_segmentation(KINDS[arr.dtype], p(src), *arr.shape, *factor, p(out)) == n
+    from chunkflow_b200._native import DTYPE_BOOL, DTYPE_U32, DTYPE_U64
+    dtype = (DTYPE_BOOL, DTYPE_U32, DTYPE_U64)[KINDS[arr.dtype]]
+    f, work = (C.c_int64 * 3)(*factor), C.c_int64()
+    assert lib.cfb_downsample_workspace(dtype, *arr.shape, C.byref(f), None, C.byref(work)) == 0, lib.cfb_last_error()
+    ws = np.zeros(max(work.value, 1), np.uint8)
+    assert lib.cfb_downsample_segmentation_device(p(src), dtype, *arr.shape, C.byref(f), p(ws), p(out), None) == 0, lib.cfb_last_error()
     np.testing.assert_array_equal(src, arr)   # the input is only read
     return out
 
@@ -274,7 +279,7 @@ def test_emulation_average_both_paths(emu, factor, shape, offset):
     a[0, 0, :8] = 255
     o = tuple(-(-s // k) for s, k in zip(shape, factor))
     out = aligned(o, np.uint8)
-    path = emu.emu_average(C.c_void_p(a.ctypes.data), *shape, *factor, C.c_void_p(out.ctypes.data))
+    path = emu_average(emu, a, factor, out)
     assert path == (factor[1:] == (2, 2) and factor[0] <= 2 and shape[2] % 16 == 0 and offset == 0)
     np.testing.assert_array_equal(out, DO.downsample_with_averaging(a, factor))
 

@@ -1,19 +1,18 @@
 """`evaluate-segmentation` (DESIGN.md section 0, row f5; reference chunk/segmentation.py:33-67 -> lib/gala/evaluate.py) on the CPU:
 the numpy oracle (oracle/evaluation_oracle.py) against golden vectors of the REAL reference
 (tests/golden/evaluate_reference.npz, made by tests/golden/make_golden_evaluate.py) and, where the reference tree exists,
-against the live reference; the device code of csrc/evaluate_kernels.cuh and the host scoring code of csrc/evaluate_scores.h,
-compiled for the host behind a one-thread CUDA shim (tests/host_emulation/evaluate_emulation.cpp), against the oracle."""
+against the live reference; csrc/evaluate.cu and its host scoring code (csrc/evaluate_scores.h), compiled for the host behind a
+one-lane CUDA shim (tests/host_emulation), against the oracle."""
 import ctypes as C
 import io
 import os
-import shutil
-import subprocess
 import warnings
 from contextlib import redirect_stdout
 
 import numpy as np
 import pytest
 
+import host_emulation
 from oracle import evaluation_oracle as EV
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -135,17 +134,14 @@ def test_oracle_is_invariant_under_relabelling_with_wide_ids():
 # ------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if gxx is None:
-        pytest.skip("g++ not available")
-    out = tmp_path_factory.mktemp("ev_emu") / "libev_emu.so"
-    src = os.path.join(ROOT, "tests", "host_emulation", "evaluate_emulation.cpp")
-    subprocess.run([gxx, "-O2", "-std=c++17", "-shared", "-fPIC", "-Wno-unknown-pragmas", "-I", os.path.join(ROOT, "include"), src,
-                    "-o", str(out)], check=True)
-    lib = C.CDLL(str(out))
-    lib.emu_evaluate.restype = C.c_int64
+    lib = host_emulation.build("evaluate", tmp_path_factory)
     from chunkflow_b200._native import SegScores
-    assert lib.emu_scores_size() == C.sizeof(SegScores)
+    i32, i64, vp = C.c_int32, C.c_int64, C.c_void_p
+    lib.cfb_evaluate_workspace.argtypes = [i64]
+    lib.cfb_evaluate_workspace.restype = i64
+    lib.cfb_contingency_device.argtypes = [vp, i32, vp, i32, i64, i64, i64, vp, i64, C.POINTER(i64), vp]
+    lib.cfb_contingency_scores.argtypes = [vp, i64, C.c_double, C.POINTER(SegScores), vp]   # refuses another struct_size
+    lib.cfb_contingency_read.argtypes = [vp, i64, i64, vp, vp, vp, vp]
     return lib
 
 
@@ -157,14 +153,22 @@ def emu_evaluate(lib, seg, gt, size_threshold, slots=None):
         slots = 32
         while slots < 4 * seg.size:
             slots <<= 1
+    from chunkflow_b200._native import DTYPE_U8, DTYPE_U32, DTYPE_U64, ERR_CAPACITY
+    dtype = {1: DTYPE_U8, 4: DTYPE_U32, 8: DTYPE_U64}
     s, g, c = np.empty(slots, np.uint64), np.empty(slots, np.uint64), np.empty(slots, np.uint32)
-    out = SegScores()
+    out = SegScores(struct_size=C.sizeof(SegScores))
     p = lambda a: C.c_void_p(a.ctypes.data)
-    n = lib.emu_evaluate(p(seg), seg.dtype.itemsize, p(gt), gt.dtype.itemsize, C.c_int64(seg.size), C.c_int64(slots),
-                         C.c_double(size_threshold), p(s), p(g), p(c), C.byref(out))
-    if n < 0:
-        return int(n), None, None
-    return int(n), (s[:n], g[:n], c[:n]), out.as_dict()
+    work = np.zeros(lib.cfb_evaluate_workspace(slots) // 8, np.uint64)
+    n = C.c_int64()
+    rc = lib.cfb_contingency_device(p(seg), dtype[seg.dtype.itemsize], p(gt), dtype[gt.dtype.itemsize], 1, 1, seg.size, p(work), slots,
+                                    C.byref(n), None)
+    if rc == ERR_CAPACITY:
+        return -1, None, None
+    assert rc == 0, lib.cfb_last_error()
+    assert lib.cfb_contingency_scores(p(work), slots, size_threshold, C.byref(out), None) == 0, lib.cfb_last_error()
+    n = n.value
+    assert lib.cfb_contingency_read(p(work), slots, n, p(s), p(g), p(c), None) == 0, lib.cfb_last_error()
+    return n, (s[:n], g[:n], c[:n]), out.as_dict()
 
 
 def assert_emulation_matches_oracle(lib, seg, gt, thr):

@@ -1,16 +1,15 @@
 """`gaussian-filter` and the median filter (DESIGN.md section 0, row f8) on the CPU: the numpy oracle (oracle/filters_oracle.py)
 against live scipy.ndimage and against golden vectors of the reference's own three callers (tests/golden/filters_reference.npz,
-made by tests/golden/make_golden_filters.py); the device code of csrc/filter_kernels.cuh, compiled for the host behind a
-one-lane CUDA shim (tests/host_emulation/filters_emulation.cpp), against the oracle; the refusals; the command's options."""
+made by tests/golden/make_golden_filters.py); csrc/filters.cu, compiled for the host behind a one-lane CUDA shim
+(tests/host_emulation), against the oracle; the refusals; the command's options."""
 import ctypes as C
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 from scipy import ndimage as ndi
 
+import host_emulation
 from oracle import filters_oracle as FO
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -144,18 +143,11 @@ def test_oracle_refusals():
 # ------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if gxx is None:
-        pytest.skip("g++ not available")
-    out = tmp_path_factory.mktemp("flt_emu") / "libflt_emu.so"
-    src = os.path.join(ROOT, "tests", "host_emulation", "filters_emulation.cpp")
-    subprocess.run([gxx, "-O2", "-std=c++17", "-ffp-contract=off", "-shared", "-fPIC", "-Wno-unknown-pragmas", src, "-o", str(out)],
-                   check=True)
-    lib = C.CDLL(str(out))
-    i64, vp = C.c_int64, C.c_void_p
-    lib.emu_gaussian.argtypes = [C.c_int, vp, i64, i64, i64, i64, vp, C.c_int, vp, C.c_int, vp, C.c_int, i64]
-    lib.emu_median.argtypes = [C.c_int, vp, i64, i64, i64, i64, vp, C.c_int, vp]
-    lib.emu_median.restype = C.c_int
+    lib = host_emulation.build("filters", tmp_path_factory)
+    i32, i64, vp = C.c_int32, C.c_int64, C.c_void_p
+    lib.emu_gaussian.argtypes = [i32, vp, i64, i64, i64, i64, vp, i32, vp, i32, vp, i32, i64]
+    lib.cfb_median_filter_device.argtypes = [vp, i32, i64, i64, i64, i64, vp, i32, vp, vp]
+    lib.emu_median_path.argtypes = [vp]
     return lib
 
 
@@ -167,7 +159,8 @@ def emu_gaussian(lib, arr, weights, batch):
     args = []
     for w in keep:
         args += [None, 0] if w is None else [C.c_void_p(w.ctypes.data), len(w) - 1]
-    lib.emu_gaussian(0 if a.dtype == np.uint8 else 1, C.c_void_p(a.ctypes.data), *czyx, *args, batch)
+    rc = lib.emu_gaussian(0 if a.dtype == np.uint8 else 1, C.c_void_p(a.ctypes.data), *czyx, *args, batch)
+    assert rc == 0, lib.cfb_last_error()
     return a
 
 
@@ -210,9 +203,10 @@ def emu_median(lib, arr, size, mode):
     ext = FO.per_axis(size, a.ndim, "size")
     s = np.array(([1] + ext) if a.ndim == 3 else ext, np.int64)
     out = np.zeros_like(a)
-    path = lib.emu_median(0 if a.dtype == np.uint8 else 1, C.c_void_p(a.ctypes.data), *czyx, C.c_void_p(s.ctypes.data),
-                          FO.MODES[mode], C.c_void_p(out.ctypes.data))
-    return out, path
+    rc = lib.cfb_median_filter_device(C.c_void_p(a.ctypes.data), 0 if a.dtype == np.uint8 else 1, *czyx, C.c_void_p(s.ctypes.data),
+                                      FO.MODES[mode], C.c_void_p(out.ctypes.data), None)
+    assert rc == 0, lib.cfb_last_error()
+    return out, lib.emu_median_path(C.c_void_p(s.ctypes.data))
 
 
 @pytest.mark.parametrize("dtype", [np.uint8, np.float32])

@@ -1,18 +1,16 @@
 """Segmentation clean-up (DESIGN.md section 0, row f6; reference chunk/segmentation.py:69-109, flow/flow.py:2015-2050) on the CPU:
 the numpy oracle (oracle/relabel_oracle.py) against golden vectors of the REAL reference's methods
 (tests/golden/relabel_reference.npz, made by tests/golden/make_golden_relabel.py) and, where the reference tree exists, against
-the live reference; the device code of csrc/label_table.cuh, compiled for the host behind a one-lane CUDA shim
-(tests/host_emulation/relabel_emulation.cpp), against the oracle; the command's option names; the wrappers' argument checks."""
+the live reference; csrc/relabel.cu, compiled for the host behind a one-lane CUDA shim (tests/host_emulation), against the oracle; the command's option names; the wrappers' argument checks."""
 import ctypes as C
 import json
 import os
 import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import host_emulation
 from oracle import relabel_oracle as RO
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -139,15 +137,24 @@ def test_selected_ids_parsing(tmp_path, capsys):
 # ------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if gxx is None:
-        pytest.skip("g++ not available")
-    out = tmp_path_factory.mktemp("lt_emu") / "liblt_emu.so"
-    src = os.path.join(ROOT, "tests", "host_emulation", "relabel_emulation.cpp")
-    subprocess.run([gxx, "-O2", "-std=c++17", "-shared", "-fPIC", "-Wno-unknown-pragmas", src, "-o", str(out)], check=True)
-    lib = C.CDLL(str(out))
-    lib.emu_relabel.restype = C.c_int64
+    lib = host_emulation.build("relabel", tmp_path_factory)
+    i32, i64, vp, pi64 = C.c_int32, C.c_int64, C.c_void_p, C.POINTER(C.c_int64)
+    lib.cfb_label_table_workspace.argtypes = [i64, i64]
+    lib.cfb_label_table_workspace.restype = i64
+    lib.cfb_label_table_device.argtypes = [vp, i32, i64, i64, i64, vp, i64, pi64, vp]
+    lib.cfb_label_table_read.argtypes = [vp, i64, i64, vp, vp, vp, vp]
+    lib.cfb_label_table_plan.argtypes = [vp, i64, i64, i32, i64, vp, i64, i32, C.c_uint64, pi64, pi64, C.POINTER(C.c_uint64), vp]
+    lib.cfb_label_apply_device.argtypes = [vp, i32, i64, vp, i64, vp, i32, vp]
     return lib
+
+
+def aligned_copy(arr):
+    """A copy of ``arr`` that starts on a 16-byte boundary, as the library requires."""
+    buf = np.zeros(arr.nbytes + 16, np.uint8)
+    start = (-buf.ctypes.data) % 16
+    out = buf[start:start + arr.nbytes].view(arr.dtype).reshape(arr.shape)
+    out[...] = arr
+    return out
 
 
 def emu_relabel(lib, arr, dust=None, keep=None, renumber=False, base_id=0, slots=None, in_place=False):
@@ -158,18 +165,28 @@ def emu_relabel(lib, arr, dust=None, keep=None, renumber=False, base_id=0, slots
         slots = 32
         while slots < 4 * arr.size:
             slots <<= 1
+    from chunkflow_b200._native import DTYPE_U8, DTYPE_U32, DTYPE_U64, ERR_CAPACITY
+    dtype = {1: DTYPE_U8, 4: DTYPE_U32, 8: DTYPE_U64}[arr.dtype.itemsize]
     ids, counts, first = np.empty(slots, np.uint64), np.empty(slots, np.uint32), np.empty(slots, np.uint32)
-    src = arr.copy()
-    out = src if in_place else np.zeros(arr.shape, np.uint64 if renumber else arr.dtype)
-    info = np.zeros(3, np.uint64)
+    src = aligned_copy(arr)
+    out = src if in_place else aligned_copy(np.zeros(arr.shape, np.uint64 if renumber else arr.dtype))
     keep_arr = None if keep is None else np.ascontiguousarray(keep, np.uint64)
     p = lambda a: C.c_void_p(a.ctypes.data)
-    n = lib.emu_relabel(p(src), arr.dtype.itemsize, C.c_int64(arr.size), C.c_int64(slots), int(dust is not None),
-                        C.c_int64(dust or 0), p(keep_arr) if keep_arr is not None and keep_arr.size else None,
-                        C.c_int64(-1 if keep_arr is None else keep_arr.size), int(renumber), C.c_uint64(base_id), p(ids), p(counts),
-                        p(first), p(out), p(info))
-    if n < 0:
-        return int(n), None, None, None
+    work = np.zeros(-(-lib.cfb_label_table_workspace(arr.size, slots) // 8), np.uint64)
+    n, dust_n, survivors, new_max = C.c_int64(), C.c_int64(), C.c_int64(), C.c_uint64()
+    rc = lib.cfb_label_table_device(p(src), dtype, 1, 1, arr.size, p(work), slots, C.byref(n), None)
+    if rc == ERR_CAPACITY:
+        return -1, None, None, None
+    assert rc == 0, lib.cfb_last_error()
+    n = n.value
+    assert lib.cfb_label_table_read(p(work), slots, n, p(ids), p(counts), p(first), None) == 0, lib.cfb_last_error()
+    assert lib.cfb_label_table_plan(p(work), slots, arr.size, int(dust is not None), dust or 0,
+                                    p(keep_arr) if keep_arr is not None and keep_arr.size else None,
+                                    -1 if keep_arr is None else keep_arr.size, int(renumber), base_id, C.byref(dust_n),
+                                    C.byref(survivors), C.byref(new_max), None) == 0, lib.cfb_last_error()
+    assert lib.cfb_label_apply_device(p(src), dtype, arr.size, p(work), slots, p(out), DTYPE_U64 if renumber else dtype,
+                                      None) == 0, lib.cfb_last_error()
+    info = (dust_n.value, survivors.value, new_max.value)
     if not in_place:
         np.testing.assert_array_equal(src, arr)   # the input is only read
     return int(n), (ids[:n], counts[:n], first[:n]), out, tuple(int(v) for v in info)

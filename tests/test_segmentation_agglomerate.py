@@ -2,8 +2,7 @@
 
 waterz is absent from the reference tree and from this image: the oracle restates its published algorithm ("parity unpinned",
 oracle/agglomeration_oracle.py).  On the CPU: the oracle against its own statement-by-statement form of the sequential
-watershed, the device code of csrc/watershed_kernels.cuh compiled for the host behind a one-thread CUDA shim
-(tests/host_emulation/ws_emulation.cpp) against the oracle, and the native library's host merge loop against the oracle.
+watershed, csrc/segmentation.cu compiled for the host behind a one-lane CUDA shim (tests/host_emulation) against the oracle, and the native library's host merge loop against the oracle.
 On the GPU: the CUDA kernels through the C ABI against the oracle, plus size-independent properties on a larger volume."""
 import ctypes as C
 import os
@@ -13,6 +12,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import host_emulation
 from oracle import agglomeration_oracle as A
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -87,14 +87,16 @@ def test_plateau_interiors_are_where_the_two_forms_may_differ():
 # ------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    gxx = shutil.which("g++")
-    if gxx is None:
-        pytest.skip("g++ not available")
-    out = tmp_path_factory.mktemp("ws_emu") / "libws_emu.so"
-    src = os.path.join(ROOT, "tests", "host_emulation", "ws_emulation.cpp")
-    subprocess.run([gxx, "-O2", "-std=c++17", "-shared", "-fPIC", "-Wno-unknown-pragmas", src, "-o", str(out)], check=True)
-    lib = C.CDLL(str(out))
-    lib.emu_region_graph.restype = C.c_int64
+    lib = host_emulation.build("ws", tmp_path_factory)
+    i32, i64, vp = C.c_int32, C.c_int64, C.c_void_p
+    lib.cfb_watershed_workspace.argtypes = [i64, i64, i64]
+    lib.cfb_watershed_workspace.restype = i64
+    lib.cfb_watershed_device.argtypes = [vp, i32, i64, i64, i64, C.c_float, C.c_float, vp, vp, C.POINTER(C.c_uint32), vp]
+    lib.cfb_region_graph_workspace.argtypes = [i64]
+    lib.cfb_region_graph_workspace.restype = i64
+    lib.cfb_region_graph_device.argtypes = [vp, i32, vp, i64, i64, i64, vp, i64, C.POINTER(i64), vp]
+    lib.cfb_region_graph_read.argtypes = [vp, i64, i64, vp, vp, vp, vp, vp]
+    lib.cfb_relabel_device.argtypes = [vp, i64, vp, i64, vp, vp]
     return lib
 
 
@@ -106,8 +108,10 @@ def _emu_watershed(lib, affs, flip):
     affs = np.ascontiguousarray(affs, np.float32)
     z, y, x = affs.shape[1:]
     out = np.empty((z, y, x), np.uint32)
-    n = lib.emu_watershed(_p(affs), C.c_int(flip), C.c_int64(z), C.c_int64(y), C.c_int64(x), C.c_float(LOW), C.c_float(HIGH), _p(out))
-    return out, n
+    work = np.zeros(lib.cfb_watershed_workspace(z, y, x) // 4, np.uint32)
+    n = C.c_uint32()
+    assert lib.cfb_watershed_device(_p(affs), flip, z, y, x, LOW, HIGH, _p(out), _p(work), C.byref(n), None) == 0, lib.cfb_last_error()
+    return out, n.value
 
 
 def _emu_region_graph(lib, affs, flip, frag, slots):
@@ -115,10 +119,16 @@ def _emu_region_graph(lib, affs, flip, frag, slots):
     z, y, x = frag.shape
     u, v = np.empty(slots, np.uint32), np.empty(slots, np.uint32)
     s, c = np.empty(slots, np.uint64), np.empty(slots, np.uint32)
-    n = lib.emu_region_graph(_p(affs), C.c_int(flip), _p(frag), C.c_int64(z), C.c_int64(y), C.c_int64(x), C.c_int64(slots),
-                             _p(u), _p(v), _p(s), _p(c))
-    k = max(int(n), 0)
-    return n, u[:k], v[:k], s[:k], c[:k]
+    from chunkflow_b200._native import ERR_CAPACITY
+    work = np.zeros(lib.cfb_region_graph_workspace(slots) // 8, np.uint64)
+    n = C.c_int64()
+    rc = lib.cfb_region_graph_device(_p(affs), flip, _p(frag), z, y, x, _p(work), slots, C.byref(n), None)
+    if rc == ERR_CAPACITY:
+        return -1, u[:0], v[:0], s[:0], c[:0]
+    assert rc == 0, lib.cfb_last_error()
+    n = n.value
+    assert lib.cfb_region_graph_read(_p(work), slots, n, _p(u), _p(v), _p(s), _p(c), None) == 0, lib.cfb_last_error()
+    return n, u[:n], v[:n], s[:n], c[:n]
 
 
 def test_kernel_logic_on_the_host_against_the_oracle(emu):
@@ -149,7 +159,7 @@ def test_whole_operator_with_emulated_voxel_passes_and_the_native_merge_loop(emu
         cnt, u, v, s, c = _emu_region_graph(emu, a, 1, frag, 1 << 14)
         root = _native.agglomerate_edges_host(n + 1, u, v, s, c, thr)
         seg = np.empty_like(frag)
-        emu.emu_relabel(_p(frag), C.c_int64(frag.size), _p(root), C.c_uint32(root.size), _p(seg))
+        assert emu.cfb_relabel_device(_p(frag), frag.size, _p(root), root.size, _p(seg), None) == 0
         assert np.array_equal(seg.astype(np.uint64), A.agglomerate(a, thr, flip_channel=True)), (seed, kind)
 
 
