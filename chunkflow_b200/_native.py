@@ -19,6 +19,7 @@ PRECISION_F32_SIMT, PRECISION_F16X3_UMMA, PRECISION_F16_UMMA, PRECISION_F16F8_UM
 DTYPE_U8, DTYPE_F32, DTYPE_U32, DTYPE_U64, DTYPE_BOOL = 0, 1, 2, 3, 4
 AUGMENT_NONE, AUGMENT_REFERENCE, AUGMENT_SPATIAL = 0, 1, 2
 QUANTIZE_XY, QUANTIZE_Z = 0, 1
+HIST_SLOTS_PER_SLOT = 2   # cfb_region_graph_hist_device: the bin table has 2 x table_slots slots
 
 # every symbol include/chunkflow_b200.h declares
 EXPORTS = (
@@ -32,6 +33,7 @@ EXPORTS = (
     "cfb_connected_components_device", "cfb_connected_components_workspace",
     "cfb_watershed_workspace", "cfb_watershed_device", "cfb_region_graph_workspace", "cfb_region_graph_device",
     "cfb_region_graph_read", "cfb_agglomerate_edges_host", "cfb_relabel_device",
+    "cfb_region_graph_hist_workspace", "cfb_region_graph_hist_device", "cfb_region_graph_hist_read", "cfb_agglomerate_quantile_host",
     "cfb_evaluate_workspace", "cfb_contingency_device", "cfb_contingency_scores", "cfb_contingency_read",
     "cfb_label_table_workspace", "cfb_label_table_device", "cfb_label_table_read", "cfb_label_table_plan",
     "cfb_label_apply_device", "cfb_downsample_average_device", "cfb_downsample_workspace", "cfb_downsample_segmentation_device",
@@ -147,6 +149,11 @@ def load() -> C.CDLL:
     lib.cfb_region_graph_read.argtypes = [vp, i64, i64, vp, vp, vp, vp, vp]
     lib.cfb_agglomerate_edges_host.argtypes = [i64, i64, vp, vp, vp, vp, C.c_float, vp]
     lib.cfb_relabel_device.argtypes = [vp, i64, vp, i64, vp, vp]
+    lib.cfb_region_graph_hist_workspace.argtypes = [i64]
+    lib.cfb_region_graph_hist_workspace.restype = i64
+    lib.cfb_region_graph_hist_device.argtypes = [vp, i32, vp, i64, i64, i64, i32, vp, i64, C.POINTER(i64), C.POINTER(i64), vp]
+    lib.cfb_region_graph_hist_read.argtypes = [vp, i64, i64, i64, vp, vp, vp, vp, vp, vp, vp]
+    lib.cfb_agglomerate_quantile_host.argtypes = [i64, i64, vp, vp, vp, vp, vp, vp, i32, i32, i32, C.c_float, vp]
     lib.cfb_evaluate_workspace.argtypes = [i64]
     lib.cfb_evaluate_workspace.restype = i64
     lib.cfb_contingency_device.argtypes = [vp, i32, vp, i32, i64, i64, i64, vp, i64, C.POINTER(i64), vp]
@@ -266,6 +273,49 @@ def agglomerate_edges_host(num_nodes: int, u, v, sum_fixed, count, threshold: fl
         raise ValueError("edge arrays must be one-dimensional and of equal length")
     root = np.empty(int(num_nodes), np.uint32)
     check(load().cfb_agglomerate_edges_host(int(num_nodes), int(u.size), _ptr(u), _ptr(v), _ptr(s), _ptr(c), float(threshold), _ptr(root)))
+    return root
+
+
+def region_graph_hist_workspace(table_slots: int) -> int:
+    return int(load().cfb_region_graph_hist_workspace(int(table_slots)))
+
+
+def region_graph_hist_device(d_affs: int, flip_channel: bool, d_fragments: int, zyx, bins: int, d_workspace: int, table_slots: int,
+                             stream: int = 0):
+    """-> (edges, histogram entries); raises NativeError with code ERR_CAPACITY when a table is too small."""
+    n, nh = C.c_int64(), C.c_int64()
+    check(load().cfb_region_graph_hist_device(C.c_void_p(d_affs), int(bool(flip_channel)), C.c_void_p(d_fragments),
+                                              *(int(v) for v in zyx), int(bins), C.c_void_p(d_workspace), int(table_slots),
+                                              C.byref(n), C.byref(nh), C.c_void_p(stream)))
+    return int(n.value), int(nh.value)
+
+
+def region_graph_hist_read(d_workspace: int, table_slots: int, num_edges: int, num_entries: int, stream: int = 0):
+    """-> (u, v, offsets, bins, counts, maxima) host arrays, edges sorted by (u, v), each run of bins sorted."""
+    u, v, mx = np.empty(num_edges, np.uint32), np.empty(num_edges, np.uint32), np.empty(num_edges, np.float32)
+    off = np.empty(num_edges + 1, np.uint64)
+    b, c = np.empty(num_entries, np.uint8), np.empty(num_entries, np.uint32)
+    check(load().cfb_region_graph_hist_read(C.c_void_p(d_workspace), int(table_slots), int(num_edges), int(num_entries), _ptr(u),
+                                            _ptr(v), _ptr(off), _ptr(b), _ptr(c), _ptr(mx), C.c_void_p(stream)))
+    return u, v, off, b, c, mx
+
+
+def agglomerate_quantile_host(num_nodes: int, u, v, offsets, bins, counts, maxima, threshold: float, quantile: int, num_bins: int,
+                              init_with_max: bool) -> np.ndarray:
+    """The merge loop with a histogram-quantile score, on the host (no GPU involved) -> root_of (num_nodes,) uint32."""
+    u = np.ascontiguousarray(u, np.uint32); v = np.ascontiguousarray(v, np.uint32)
+    off = np.ascontiguousarray(offsets, np.uint64)
+    b = np.ascontiguousarray(bins, np.uint8); c = np.ascontiguousarray(counts, np.uint32)
+    if not (u.shape == v.shape and u.ndim == 1 and off.shape == (u.size + 1,) and b.shape == c.shape and b.ndim == 1):
+        raise ValueError("edge arrays must be one-dimensional, offsets one longer than the edges, bins as long as counts")
+    if off[-1] != b.size:
+        raise ValueError("offsets[-1] must be the number of bins")
+    mx = np.ascontiguousarray(maxima if maxima is not None else np.zeros(u.size), np.float32)
+    if mx.shape != u.shape:
+        raise ValueError("one maximum per edge")
+    root = np.empty(int(num_nodes), np.uint32)
+    check(load().cfb_agglomerate_quantile_host(int(num_nodes), int(u.size), _ptr(u), _ptr(v), _ptr(off), _ptr(b), _ptr(c), _ptr(mx),
+                                               int(quantile), int(num_bins), int(bool(init_with_max)), float(threshold), _ptr(root)))
     return root
 
 

@@ -23,7 +23,8 @@ brings a uint8 thumbnail (or nothing) back instead of the 12-byte-per-voxel affi
 """
 from __future__ import annotations
 
-from typing import Optional, Sequence
+import re
+from typing import NamedTuple, Optional, Sequence
 
 import numpy as np
 
@@ -148,6 +149,38 @@ def _grown_table(device, slots: int, workspace_bytes, build, what: str):
         slots <<= 2
         if slots >= 1 << 31:
             raise RuntimeError(f"{what} than the table can hold")
+
+
+MEAN_AFFINITY = 'OneMinus<MeanAffinity<RegionGraphType, ScoreValue>>'
+_HIST_QUANTILE = re.compile(r'OneMinus<HistogramQuantileAffinity<RegionGraphType,([+-]?\d+),ScoreValue,([+-]?\d+)(?:,(\w+))?>>')
+
+
+class HistogramQuantile(NamedTuple):
+    """``OneMinus<HistogramQuantileAffinity<RegionGraphType, quantile, ScoreValue, bins, init_with_max>>``"""
+    quantile: int
+    bins: int
+    init_with_max: bool
+
+
+def parse_scoring_function(scoring_function: str) -> Optional[HistogramQuantile]:
+    """None for waterz's mean affinity, a :class:`HistogramQuantile` for its histogram-quantile family (whitespace ignored;
+    an omitted init_with_max means true, waterz's default).  Any other scoring function raises NotImplementedError, one of the
+    family with a quantile outside 0..100, bins outside 2..256 or init_with_max other than true / false ValueError."""
+    s = re.sub(r'\s', '', scoring_function) if isinstance(scoring_function, str) else None
+    if s == MEAN_AFFINITY.replace(' ', ''):
+        return None
+    m = _HIST_QUANTILE.fullmatch(s) if s is not None else None
+    if m is None:
+        raise NotImplementedError(f'scoring function {scoring_function!r}: only {MEAN_AFFINITY} and '
+                                  'OneMinus<HistogramQuantileAffinity<RegionGraphType, Q, ScoreValue, B[, I]>> are implemented')
+    q, bins, init = int(m.group(1)), int(m.group(2)), m.group(3)
+    if not 0 <= q <= 100:
+        raise ValueError(f'the quantile must be in 0..100, not {q}')
+    if not 2 <= bins <= 256:
+        raise ValueError(f'the number of bins must be in 2..256, not {bins}')
+    if init not in (None, 'true', 'false'):
+        raise ValueError(f'init_with_max must be true or false, not {init}')
+    return HistogramQuantile(q, bins, init != 'false')
 
 
 class DeviceChunk:
@@ -328,10 +361,16 @@ class DeviceChunk:
         out.num_components = n
         return out
 
-    def region_graph(self, fragments: "DeviceChunk", flip_channel: bool = True, num_fragments: Optional[int] = None):
+    def region_graph(self, fragments: "DeviceChunk", flip_channel: bool = True, num_fragments: Optional[int] = None,
+                     histogram_bins: Optional[int] = None):
         """(u, v, sum_fixed, count) host arrays, one entry per pair of touching fragments, sorted by (u, v): the sum (2^-30
         fixed point) and number of the affinities on the faces between them (waterz's region graph with MeanAffinity
-        statistics).  The hash table is sized from the fragment count and grown on overflow."""
+        statistics).  The hash table is sized from the fragment count and grown on overflow.
+
+        With ``histogram_bins`` B (2..256): (u, v, offsets, bins, counts, maxima) instead, the statistics of waterz's
+        HistogramQuantileAffinity -- edge i counts ``counts[offsets[i]:offsets[i+1]]`` faces in the increasing ``bins`` of
+        the same slice (bin = min(int(a * B), B - 1) of the clamped affinity, float32), and ``maxima[i]`` is its largest
+        clamped affinity."""
         torch = _torch()
         t = self._affinity_tensor()
         f = fragments.tensor
@@ -343,6 +382,8 @@ class DeviceChunk:
         slots = 1 << 16
         while slots < 16 * num_fragments:
             slots <<= 1
+        if histogram_bins is not None:
+            return self._region_graph_hist(t, f, flip_channel, int(histogram_bins), slots)
         with self._on_device():
             work, slots, n = _grown_table(
                 t.device, slots, _native.region_graph_workspace,
@@ -351,14 +392,33 @@ class DeviceChunk:
                 "region graph: more fragment pairs")
             return _native.region_graph_read(work.data_ptr(), slots, n, self._stream())
 
+    def _region_graph_hist(self, t, f, flip_channel, bins, slots):
+        found = {}
+
+        def build(work, slots):
+            found["edges"], found["entries"] = _native.region_graph_hist_device(
+                t.data_ptr(), flip_channel, f.data_ptr(), tuple(f.shape), bins, work.data_ptr(), slots, self._stream())
+            # the bin table has HIST_SLOTS_PER_SLOT times as many slots: keep both at most half full
+            return max(found["edges"], -(-found["entries"] // _native.HIST_SLOTS_PER_SLOT))
+
+        with self._on_device():
+            work, slots, _ = _grown_table(t.device, slots, _native.region_graph_hist_workspace, build,
+                                          "region graph: more fragment pairs or histogram bins")
+            return _native.region_graph_hist_read(work.data_ptr(), slots, found["edges"], found["entries"], self._stream())
+
     def agglomerate(self, threshold: float = 0.7, aff_threshold_low: float = 0.001, aff_threshold_high: float = 0.9999,
-                    fragments: Optional["DeviceChunk"] = None, flip_channel: bool = True) -> "DeviceChunk":
-        """Mean-affinity agglomeration including the watershed step (reference plugins/agglomerate.py:8-48 ->
-        ``waterz.agglomerate`` with ``OneMinus<MeanAffinity<RegionGraphType, ScoreValue>>``): fragments (watershed, unless
-        given) -> region graph -> merge edges in order of increasing ``1 - mean affinity`` until ``threshold`` -> relabel.
-        The voxel passes are CUDA kernels; the merge loop over the fragment graph runs in the native library on the host
-        (as waterz's does).  Returns a (z,y,x) uint32 segmentation whose ids are the surviving fragment ids."""
+                    fragments: Optional["DeviceChunk"] = None, flip_channel: bool = True,
+                    scoring_function: str = MEAN_AFFINITY) -> "DeviceChunk":
+        """Agglomeration including the watershed step (reference plugins/agglomerate.py:8-48 -> ``waterz.agglomerate``):
+        fragments (watershed, unless given) -> region graph -> merge edges in order of increasing score until
+        ``threshold`` -> relabel.  ``scoring_function``: waterz's ``OneMinus<MeanAffinity<RegionGraphType, ScoreValue>>``
+        (1 - mean affinity) or ``OneMinus<HistogramQuantileAffinity<RegionGraphType, Q, ScoreValue, B[, I]>>`` (1 - the
+        Q-th percentile of a B-bin histogram of the affinities; with I, 1 - the largest affinity until an edge is pooled),
+        see :func:`parse_scoring_function`.  The voxel passes are CUDA kernels; the merge loop over the fragment graph runs
+        in the native library on the host (as waterz's does).  Returns a (z,y,x) uint32 segmentation whose ids are the
+        surviving fragment ids."""
         torch = _torch()
+        hq = parse_scoring_function(scoring_function)
         t = self._affinity_tensor()
         if fragments is None:
             fragments = self.watershed(aff_threshold_low, aff_threshold_high, flip_channel)
@@ -370,8 +430,12 @@ class DeviceChunk:
             num = int(f.view(torch.int32).max().item()) if f.numel() else 0
         if num < 0:
             raise ValueError("fragment ids must be below 2^31")
-        u, v, s, c = self.region_graph(fragments, flip_channel, num)
-        root = _native.agglomerate_edges_host(num + 1, u, v, s, c, threshold)
+        if hq is None:
+            u, v, s, c = self.region_graph(fragments, flip_channel, num)
+            root = _native.agglomerate_edges_host(num + 1, u, v, s, c, threshold)
+        else:
+            u, v, off, b, c, mx = self.region_graph(fragments, flip_channel, num, histogram_bins=hq.bins)
+            root = _native.agglomerate_quantile_host(num + 1, u, v, off, b, c, mx, threshold, hq.quantile, hq.bins, hq.init_with_max)
         d_root = torch.from_numpy(root.view(np.int32)).to(t.device)
         seg = torch.empty(f.shape, dtype=torch.int32, device=t.device)
         with self._on_device():

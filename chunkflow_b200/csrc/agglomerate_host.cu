@@ -28,6 +28,26 @@
 //   * priority queue: only edges with score < threshold ever enter it.  A new entry never precedes the edge being merged, so
 //     the queue is MONOTONE: 65 536 score buckets (append-only vectors) and a small heap for the bucket being drained, which
 //     keeps the exact (score, anchor) order inside it.
+//
+// The quantile family, OneMinus<HistogramQuantileAffinity<RegionGraphType, Q, ScoreValue, B, I>> (`QuantileScoring`, rules
+// restated in oracle/agglomeration_oracle.py: agglomerate_edges_quantile): an edge carries the histogram of its faces over
+// B bins and scores 1 - (q + 0.5) / B, q the first bin whose cumulative count reaches the pivot p(n) = min(floor(Q n / 100)
+// + 1, n); with I (init_with_max), an edge never pooled scores 1 - its largest affinity.  Pooled edges add their histograms
+// and take the anchor of the one that comes first in (score, anchor) order (rule 6): then a pooled key is never below both
+// keys pooled even when its score equals the smaller score, and anchors stay unique among live edges (the faces of live
+// edges are disjoint, and an anchor is one of them).  A pooled quantile lies between the two quantiles, q1 <= q2:
+//   * p(n1 + n2) >= p1 + p2 - 1, since floor(Q (n1 + n2) / 100) >= floor(Q n1 / 100) + floor(Q n2 / 100) and n1 + n2 >= p1 + p2.
+//     Below q1 both cumulative counts fall short of their pivots, so their sum is at most p1 + p2 - 2 < p(n1 + n2): q >= q1.
+//   * p(n1 + n2) <= p1 + p2: for Q = 100 all three pivots are the totals; for Q < 100 no pivot is clamped (Q n / 100 < n)
+//     and floor(x + y) <= floor(x) + floor(y) + 1.  At q2 the two cumulative counts reach p1 + p2: q <= q2.
+// So with I = false the walk's queue is monotone as for the mean.  With I = true it is not: a pooled quantile may exceed both
+// maxima by up to one bin width (a maximum of 0.5 lies in bin 128 of 256, worth 0.50195), so a pooled edge may score below
+// both edges it pools, even below the edge being merged; the bucket queue stays exact (see BucketQueue).  The ROUNDS do not
+// run for this family at all, whatever I: rule 6 is not associative -- pooling e1 with e2 and then with e3 may keep another
+// anchor than pooling e1 with e3 first, because the first pooled score is not the smaller one -- so the walk's result
+// depends on the order in which merges pool edges, and a round, which pools all the edges of its merges at once, does not
+// reproduce it.  (With I = true the mutual-best argument and the pruning of clusters without an edge below the threshold
+// fail as well: pooling can give such a cluster one.)
 // One host core, 2.4 M fragments / 11.2 M edges of a noisy 64x512x512 map, threshold 0.5, 1.8 M merges
 // (profiles/r02c_host_merge_loop.txt): 42 s with std::unordered_map + std::vector per node + one binary heap, 11.2 s for the
 // walk alone as it is now, 3.4 s with the rounds in front on 8 threads (the rounds share every pass among worker threads;
@@ -49,16 +69,17 @@
 
 namespace {
 
+template <typename Stat>
 struct Entry {
   double score;
-  uint64_t anchor;  // smallest original (u << 32 | v) pooled into the edge: the tie rule
-  uint64_t sum;
+  uint64_t anchor;  // an original (u << 32 | v) pooled into the edge: the tie rule
+  Stat st;          // the edge's statistic when the entry was pushed (a later one makes the entry stale)
   uint32_t a, b;    // structural roots of the two clusters when the entry was pushed
-  uint32_t count;
 };
 
 struct Later {  // std::priority_queue keeps the LARGEST element on top: order by "comes later"
-  bool operator()(const Entry& x, const Entry& y) const {
+  template <typename E>
+  bool operator()(const E& x, const E& y) const {
     if (x.score != y.score) return x.score > y.score;
     return x.anchor > y.anchor;
   }
@@ -69,18 +90,20 @@ inline uint64_t edge_key(uint32_t p, uint32_t q) { return p < q ? ((uint64_t)p <
 inline double edge_score(uint64_t sum, uint32_t count) { return 1.0 - (double)sum / ((double)count * 1073741824.0); }
 
 // key 0 = never used (ids >= 1 would make key 0 impossible anyway: node 0 may not appear with itself), ~0 = tombstone
+template <typename Stat>
 class EdgeTable {
  public:
   struct Slot {
-    uint64_t key, sum, anchor;
-    uint32_t count;
+    uint64_t key;
+    Stat st;
+    uint64_t anchor;
   };
   static constexpr uint64_t kEmpty = 0, kDead = ~0ULL;
 
   explicit EdgeTable(size_t expected) {
     size_t cap = 16;
     while (cap < expected * 2 + 2) cap <<= 1;
-    slots_.assign(cap, Slot{kEmpty, 0, 0, 0});
+    slots_.assign(cap, Slot{kEmpty, Stat{}, 0});
     mask_ = cap - 1;
   }
   Slot* find(uint64_t key) {
@@ -91,13 +114,13 @@ class EdgeTable {
     }
   }
   // the key must not be present
-  void insert(uint64_t key, uint64_t sum, uint64_t anchor, uint32_t count) {
+  void insert(uint64_t key, const Stat& st, uint64_t anchor) {
     if ((used_ + 1) * 10 > slots_.size() * 7) rebuild();
     for (size_t h = hash(key) & mask_;; h = (h + 1) & mask_) {
       Slot& s = slots_[h];
       if (s.key == kEmpty || s.key == kDead) {
         if (s.key == kEmpty) ++used_;
-        s = Slot{key, sum, anchor, count};
+        s = Slot{key, st, anchor};
         ++live_;
         return;
       }
@@ -108,6 +131,11 @@ class EdgeTable {
     --live_;
   }
   void prefetch(uint64_t key) const { __builtin_prefetch(&slots_[hash(key) & mask_]); }
+  template <typename F>
+  void for_each_live(F&& f) {
+    for (Slot& s : slots_)
+      if (s.key != kEmpty && s.key != kDead) f(s);
+  }
 
  private:
   static size_t hash(uint64_t k) {
@@ -119,7 +147,7 @@ class EdgeTable {
     old.swap(slots_);
     size_t cap = old.size();
     while (cap < live_ * 2 + 2) cap <<= 1;
-    slots_.assign(cap, Slot{kEmpty, 0, 0, 0});
+    slots_.assign(cap, Slot{kEmpty, Stat{}, 0});
     mask_ = cap - 1;
     used_ = live_ = 0;
     for (const Slot& s : old)
@@ -139,8 +167,11 @@ struct Link {
 constexpr uint32_t kNil = 0xFFFFFFFFu;
 
 // Monotone priority queue over scores in [lo, hi): see the header comment.  pop() returns entries in exactly the order one
-// global heap ordered by (score, a, b) would, provided no entry is pushed with a key below the last one popped's bucket --
-// and even then it is only popped next (it joins the bucket being drained), which is what the global heap would do too.
+// global heap ordered by (score, anchor) would, whatever is pushed when: every entry of a bucket at or below the one being
+// drained is in the heap, every other entry sits in a later bucket, and the bucket index does not decrease with the score.
+// An entry pushed below the last one popped joins the heap and is popped next, as the global heap would do.  It only costs
+// speed: the heap is the whole queue while such entries come (quantile scores with init_with_max, see below).
+template <typename Entry>
 class BucketQueue {
  public:
   BucketQueue(double lo, double hi, std::vector<Entry>&& initial) : lo_(lo), scale_(hi > lo ? (double)kBuckets / (hi - lo) : 0.0) {
@@ -189,21 +220,114 @@ struct EdgeRec {   // one undirected edge between two clusters, named by their l
   uint32_t mark;
 };
 
+// The two scoring functions of the walk.  Each one has a Stat (what an edge carries), its score, a test whether a queue entry's
+// Stat is still the edge's, pool() -- edge `into` with anchor `anchor` absorbs edge `other` -- and drop(), called for an edge
+// that disappears because its two clusters merge.
+struct MeanScoring {   // OneMinus<MeanAffinity>
+  struct Stat {
+    uint64_t sum;
+    uint32_t count;
+  };
+  static Stat stat(const EdgeRec& e) { return Stat{e.sum, e.count}; }
+  static double score(const Stat& s) { return edge_score(s.sum, s.count); }
+  static bool same(const Stat& x, const Stat& y) { return x.sum == y.sum && x.count == y.count; }
+  static void pool(Stat& into, uint64_t& anchor, const Stat& other, uint64_t other_anchor) {
+    into.sum += other.sum;
+    into.count += other.count;
+    if (other_anchor < anchor) anchor = other_anchor;
+  }
+  static void drop(const Stat&) {}
+  template <typename Table>
+  static void maintain(Table&) {}
+};
+
+// OneMinus<HistogramQuantileAffinity<RegionGraphType, Q, ScoreValue, B, I>>.  An edge's histogram is a run of (count << 8 |
+// bin) words sorted by bin in one arena (sparse: a dense 1 KiB per edge would not fit graphs of 10^7 edges); a pooled edge
+// gets a new run, and the arena is compacted when dead runs outweigh the live ones.  The score is computed when the histogram
+// changes and kept with the Stat: 1 - max for an edge that was never pooled when I (init_with_max), the quantile otherwise.
+// `serial` names one state of one edge (runs move when the arena is compacted).
+struct QuantileScoring {
+  struct Stat {
+    uint64_t off;
+    uint32_t len, serial;
+    double score;
+  };
+  struct Rec {
+    uint64_t key;
+    Stat st;
+    uint64_t anchor;
+  };
+  std::vector<uint64_t> arena;
+  uint64_t live = 0;   // words of the runs of live edges
+  uint32_t next_serial = 0;
+  uint64_t q = 0;
+  int bins = 0;
+
+  static Stat stat(const Rec& e) { return e.st; }
+  static double score(const Stat& s) { return s.score; }
+  static bool same(const Stat& x, const Stat& y) { return x.serial == y.serial; }
+  // 1 - (b + 0.5) / B for the first bin b whose cumulative count reaches min(floor(Q n / 100) + 1, n)
+  double quantile(uint64_t off, uint32_t len) const {
+    uint64_t n = 0;
+    for (uint32_t i = 0; i < len; ++i) n += arena[off + i] >> 8;
+    const uint64_t pivot = std::min(q * n / 100 + 1, n);
+    uint64_t c = 0;
+    uint32_t i = 0;
+    for (; i + 1 < len; ++i)
+      if ((c += arena[off + i] >> 8) >= pivot) break;
+    return 1.0 - ((double)(arena[off + i] & 0xFF) + 0.5) / (double)bins;
+  }
+  void pool(Stat& into, uint64_t& anchor, const Stat& other, uint64_t other_anchor) {
+    if (other.score < into.score || (other.score == into.score && other_anchor < anchor)) anchor = other_anchor;
+    const uint64_t off = arena.size();
+    arena.resize(off + into.len + other.len);
+    uint64_t i = into.off, j = other.off, o = off;
+    const uint64_t ie = into.off + into.len, je = other.off + other.len;
+    while (i < ie || j < je) {
+      if (j == je || (i < ie && (arena[i] & 0xFF) < (arena[j] & 0xFF))) arena[o++] = arena[i++];
+      else if (i == ie || (arena[j] & 0xFF) < (arena[i] & 0xFF)) arena[o++] = arena[j++];
+      else { arena[o++] = arena[i++] + (arena[j++] & ~0xFFULL); }   // same bin: add the counts
+    }
+    arena.resize(o);
+    const uint32_t len = (uint32_t)(o - off);
+    live += len;
+    live -= into.len + other.len;
+    into = Stat{off, len, next_serial++, quantile(off, len)};
+  }
+  void drop(const Stat& s) { live -= s.len; }
+  template <typename Table>
+  void maintain(Table& edges) {
+    if (arena.size() < 2 * live + (1u << 20)) return;
+    std::vector<uint64_t> packed;
+    packed.reserve(live + live / 2);
+    edges.for_each_live([&](typename Table::Slot& s) {
+      const uint64_t off = packed.size();
+      packed.insert(packed.end(), arena.begin() + (std::ptrdiff_t)s.st.off, arena.begin() + (std::ptrdiff_t)(s.st.off + s.st.len));
+      s.st.off = off;
+    });
+    arena.swap(packed);
+  }
+};
+
 // The sequential walk: lowest (score, anchor) first until the threshold.  `root[i]` (identity on entry) receives, for
 // every node that is an endpoint in E or not, the label of the cluster it ends in.
-void sequential_merge(int64_t num_nodes, const std::vector<EdgeRec>& E, double thr, std::vector<uint32_t>& root) {
+template <typename Scoring, typename Rec>
+void sequential_merge(int64_t num_nodes, const std::vector<Rec>& E, double thr, std::vector<uint32_t>& root, Scoring& scoring) {
+  using Stat = typename Scoring::Stat;
+  using Slot = typename EdgeTable<Stat>::Slot;
+  using QEntry = Entry<Stat>;
   const size_t num_edges = E.size();
-  EdgeTable edges(num_edges);
+  EdgeTable<Stat> edges(num_edges);
   // initial adjacency as CSR; neighbours gained later in an overflow list per node
   std::vector<uint32_t> adj_start((size_t)num_nodes + 1, 0), adj(num_edges * 2);
-  for (const EdgeRec& e : E) {
+  for (const Rec& e : E) {
     ++adj_start[(size_t)(e.key >> 32) + 1];
     ++adj_start[(size_t)(e.key & 0xFFFFFFFFu) + 1];
   }
   for (int64_t i = 0; i < num_nodes; ++i) adj_start[i + 1] += adj_start[i];
   {
     std::vector<uint32_t> cursor(adj_start.begin(), adj_start.end() - 1);
-    for (const EdgeRec& e : E) {
+    for (const Rec& e : E) {
       const uint32_t a = (uint32_t)(e.key >> 32), b = (uint32_t)e.key;
       adj[cursor[a]++] = b;
       adj[cursor[b]++] = a;
@@ -215,28 +339,29 @@ void sequential_merge(int64_t num_nodes, const std::vector<EdgeRec>& E, double t
     pool.push_back(Link{to, head[from]});
     head[from] = (uint32_t)(pool.size() - 1);
   };
-  std::vector<Entry> initial;
+  std::vector<QEntry> initial;
   double lowest = thr;
-  for (const EdgeRec& e : E) {
-    edges.insert(e.key, e.sum, e.anchor, e.count);
-    const double sc = edge_score(e.sum, e.count);
+  for (const Rec& e : E) {
+    const Stat st = Scoring::stat(e);
+    edges.insert(e.key, st, e.anchor);
+    const double sc = scoring.score(st);
     if (sc < thr) {
-      initial.push_back(Entry{sc, e.anchor, e.sum, (uint32_t)(e.key >> 32), (uint32_t)e.key, e.count});
+      initial.push_back(QEntry{sc, e.anchor, st, (uint32_t)(e.key >> 32), (uint32_t)e.key});
       if (sc < lowest) lowest = sc;
     }
   }
-  BucketQueue queue(lowest, thr, std::move(initial));
+  BucketQueue<QEntry> queue(lowest, thr, std::move(initial));
   std::vector<uint8_t> alive((size_t)num_nodes, 1);
   std::vector<uint32_t> parent((size_t)num_nodes), label((size_t)num_nodes), entries((size_t)num_nodes);
   for (int64_t i = 0; i < num_nodes; ++i) {
     parent[i] = label[i] = (uint32_t)i;
     entries[i] = adj_start[i + 1] - adj_start[i];   // list entries (CSR run + overflow), dead ones included
   }
-  Entry e;
+  QEntry e;
   while (queue.pop(e)) {
     if (!alive[e.a] || !alive[e.b]) continue;
-    EdgeTable::Slot* it = edges.find(edge_key(e.a, e.b));
-    if (!it || it->sum != e.sum || it->count != e.count) continue;  // superseded entry
+    Slot* it = edges.find(edge_key(e.a, e.b));
+    if (!it || !Scoring::same(it->st, e.st)) continue;  // superseded entry
     // (every entry in the queue has score < threshold: nothing to test here; the loop ends when the queue runs dry)
     // the cluster with fewer list entries is merged away (`gone`) into the other (`keep`); equal: the larger root goes
     const bool a_goes = entries[e.a] < entries[e.b] || (entries[e.a] == entries[e.b] && e.a > e.b);
@@ -244,30 +369,28 @@ void sequential_merge(int64_t num_nodes, const std::vector<EdgeRec>& E, double t
     alive[gone] = 0;
     parent[gone] = keep;
     if (label[gone] < label[keep]) label[keep] = label[gone];
+    scoring.drop(it->st);
     edges.erase(it);
     auto visit = [&](uint32_t n) {
       if (n == keep || !alive[n]) return;
-      EdgeTable::Slot* eg = edges.find(edge_key(gone, n));
+      Slot* eg = edges.find(edge_key(gone, n));
       if (!eg) return;  // an entry left behind by an earlier merge
-      uint64_t sum = eg->sum, anchor = eg->anchor;
-      uint32_t cnt = eg->count;
+      Stat st = eg->st;
+      uint64_t anchor = eg->anchor;
       edges.erase(eg);
-      if (EdgeTable::Slot* ek = edges.find(edge_key(keep, n))) {
-        sum += ek->sum;
-        cnt += ek->count;
-        if (ek->anchor < anchor) anchor = ek->anchor;
-        ek->sum = sum;
-        ek->count = cnt;
-        ek->anchor = anchor;
+      if (Slot* ek = edges.find(edge_key(keep, n))) {
+        scoring.pool(ek->st, ek->anchor, st, anchor);
+        st = ek->st;
+        anchor = ek->anchor;
       } else {
-        edges.insert(edge_key(keep, n), sum, anchor, cnt);
+        edges.insert(edge_key(keep, n), st, anchor);
         link(keep, n);
         link(n, keep);
         ++entries[keep];
         ++entries[n];
       }
-      const double sc = edge_score(sum, cnt);
-      if (sc < thr) queue.push(Entry{sc, anchor, sum, keep, n, cnt});
+      const double sc = scoring.score(st);
+      if (sc < thr) queue.push(QEntry{sc, anchor, st, keep, n});
     };
     const uint32_t lo = adj_start[gone], hi = adj_start[gone + 1];
     for (uint32_t i = lo; i < hi; ++i) {   // all the cache misses of this merge in flight at once
@@ -283,6 +406,7 @@ void sequential_merge(int64_t num_nodes, const std::vector<EdgeRec>& E, double t
       visit(lk.node);
     }
     head[gone] = kNil;
+    scoring.maintain(edges);
   }
   for (int64_t i = 0; i < num_nodes; ++i) {
     uint32_t r = (uint32_t)i;
@@ -535,12 +659,77 @@ extern "C" int cfb_agglomerate_edges_host(int64_t num_nodes, int64_t num_edges, 
     // the walk on what is left: cluster labels are node ids of the contracted graph
     std::vector<uint32_t> root((size_t)num_nodes);
     for (int64_t i = 0; i < num_nodes; ++i) root[i] = (uint32_t)i;
-    if (!E.empty()) sequential_merge(num_nodes, E, thr, root);
+    MeanScoring mean;
+    if (!E.empty()) sequential_merge(num_nodes, E, thr, root, mean);
     for (int64_t i = 0; i < num_nodes; ++i) {
       uint32_t r = (uint32_t)i;
       while (parent[r] != r) r = parent[r];
       root_of[i] = root[r];
     }
+    return CFB_OK;
+  } catch (const std::invalid_argument& ex) {
+    cfb::set_last_error(ex.what());
+    return CFB_ERR_INVALID_ARGUMENT;
+  } catch (const std::exception& ex) {
+    cfb::set_last_error(ex.what());
+    return CFB_ERR_UNSUPPORTED;
+  }
+}
+
+// The quantile family: the walk alone (see the header comment for why the rounds do not run); CFB_AGGLOMERATE_MODE,
+// _THREADS and _GRAIN do not apply.
+extern "C" int cfb_agglomerate_quantile_host(int64_t num_nodes, int64_t num_edges, const uint32_t* u, const uint32_t* v,
+                                             const uint64_t* offsets, const uint8_t* bins, const uint32_t* counts, const float* maxima,
+                                             int32_t quantile, int32_t num_bins, int32_t init_with_max, float threshold,
+                                             uint32_t* root_of) {
+  try {
+    if (num_nodes < 1 || num_nodes > (int64_t)UINT32_MAX || num_edges < 0 || num_edges >= (int64_t)1 << 31 || !root_of)
+      throw std::invalid_argument("agglomerate: bad sizes");
+    if (quantile < 0 || quantile > 100 || num_bins < 2 || num_bins > 256)
+      throw std::invalid_argument("agglomerate: the quantile must be in 0..100 and the number of bins in 2..256");
+    if (num_edges && (!u || !v || !offsets || !bins || !counts || (init_with_max && !maxima)))
+      throw std::invalid_argument("agglomerate: null edge arrays");
+    QuantileScoring scoring;
+    scoring.q = (uint64_t)quantile;
+    scoring.bins = num_bins;
+    scoring.next_serial = (uint32_t)num_edges;
+    std::vector<QuantileScoring::Rec> E((size_t)num_edges);
+    if (num_edges) {
+      if (offsets[0] != 0 || offsets[num_edges] > (uint64_t)num_edges * (uint64_t)num_bins)
+        throw std::invalid_argument("agglomerate: offsets must start at 0 and hold at most num_bins bins per edge");
+      scoring.arena.resize(offsets[num_edges]);
+    }
+    bool sorted = true;
+    for (int64_t i = 0; i < num_edges; ++i) {
+      if (u[i] >= num_nodes || v[i] >= num_nodes || u[i] == v[i])
+        throw std::invalid_argument("agglomerate: edge with an id outside [0, num_nodes) or a self loop");
+      const uint64_t lo = offsets[i], hi = offsets[i + 1];
+      if (hi <= lo || hi - lo > (uint64_t)num_bins || hi > offsets[num_edges])
+        throw std::invalid_argument("agglomerate: an edge's run of bins is empty, longer than the number of bins or out of order");
+      for (uint64_t p = lo; p < hi; ++p) {
+        if (bins[p] >= num_bins || (p > lo && bins[p] <= bins[p - 1]) || !counts[p])
+          throw std::invalid_argument("agglomerate: bins must be strictly increasing, below num_bins, with non-zero counts");
+        scoring.arena[p] = ((uint64_t)counts[p] << 8) | bins[p];
+      }
+      const uint64_t key = edge_key(u[i], v[i]);
+      double sc;
+      if (init_with_max) {
+        if (!(maxima[i] >= 0.f && maxima[i] <= 1.f)) throw std::invalid_argument("agglomerate: maxima must be in [0, 1]");
+        sc = 1.0 - (double)maxima[i];
+      } else {
+        sc = scoring.quantile(lo, (uint32_t)(hi - lo));
+      }
+      E[(size_t)i] = QuantileScoring::Rec{key, QuantileScoring::Stat{lo, (uint32_t)(hi - lo), (uint32_t)i, sc}, key};
+      scoring.live += hi - lo;
+      if (i && key < E[(size_t)i - 1].key) sorted = false;
+    }
+    if (!sorted) std::sort(E.begin(), E.end(), [](const QuantileScoring::Rec& x, const QuantileScoring::Rec& y) { return x.key < y.key; });
+    for (size_t i = 1; i < E.size(); ++i)
+      if (E[i].key == E[i - 1].key) throw std::invalid_argument("agglomerate: duplicate edge");
+    std::vector<uint32_t> root((size_t)num_nodes);
+    for (int64_t i = 0; i < num_nodes; ++i) root[i] = (uint32_t)i;
+    if (!E.empty()) sequential_merge(num_nodes, E, (double)threshold, root, scoring);
+    std::copy(root.begin(), root.end(), root_of);
     return CFB_OK;
   } catch (const std::invalid_argument& ex) {
     cfb::set_last_error(ex.what());

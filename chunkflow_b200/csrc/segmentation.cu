@@ -16,6 +16,7 @@
 //   relabel   out[i] = rank[P[i]] + 1 for foreground, 0 for background
 #include <algorithm>
 #include <cstdint>
+#include <cstring>
 #include <stdexcept>
 #include <type_traits>
 #include <vector>
@@ -265,8 +266,8 @@ extern "C" int cfb_region_graph_device(const float* d_affs, int32_t flip_channel
     CFB_CUDA(cudaMemsetAsync(keys, 0, (size_t)table_slots * 16, s));     // keys + sums
     CFB_CUDA(cudaMemsetAsync(counts, 0, (size_t)table_slots * 4, s));
     CFB_CUDA(cudaMemsetAsync(info, 0, 4 * sizeof(uint32_t), s));
-    launch(rg_accumulate_kernel, grid_for(g.n), kT, 0, s, d_affs, d_fragments, g, flip_channel ? 1 : 0, keys, sums, counts,
-           (unsigned long long)(table_slots - 1), info);
+    launch(rg_accumulate_kernel<false>, grid_for(g.n), kT, 0, s, d_affs, d_fragments, g, flip_channel ? 1 : 0, keys, sums, counts,
+           (uint32_t*)nullptr, (unsigned long long)(table_slots - 1), info);
     uint32_t h_info[2] = {0, 0};
     CFB_CUDA(cudaMemcpyAsync(h_info, info, sizeof(h_info), cudaMemcpyDeviceToHost, s));
     CFB_CUDA(cudaStreamSynchronize(s));
@@ -313,6 +314,129 @@ extern "C" int cfb_region_graph_read(void* d_workspace, int64_t table_slots, int
       h_sum_fixed[i] = sm[o];
       h_count[i] = ct[o];
     }
+    return CFB_OK;
+  });
+}
+
+// ---- histogram region graph ----------------------------------------------------------------
+// workspace: pair keys | compact pair keys (8 B x table_slots) | max bits | compact max bits | slot -> compact index (4 B x
+// table_slots) | bin keys | compact bin keys (8 B x 2 table_slots) | bin counts | compact bin counts (4 B x 2 table_slots) |
+// info[8]: 0 pairs, 1 pair overflow, 2 bin entries, 3 bin overflow, 4 and 5 read cursors
+namespace cfb {
+namespace {
+constexpr int64_t kHistSlotsPerSlot = 2;
+struct HistWorkspace {
+  unsigned long long *keys, *okeys, *hkeys, *ohkeys;
+  uint32_t *maxbits, *omax, *slot_index, *hcounts, *ohcounts, *info;
+  int64_t slots, hslots;
+  HistWorkspace(void* w, int64_t table_slots) : slots(table_slots), hslots(kHistSlotsPerSlot * table_slots) {
+    keys = static_cast<unsigned long long*>(w);
+    okeys = keys + slots;
+    maxbits = reinterpret_cast<uint32_t*>(okeys + slots);
+    omax = maxbits + slots;
+    slot_index = omax + slots;
+    hkeys = reinterpret_cast<unsigned long long*>(slot_index + slots + (slots & 1));   // (8-byte aligned)
+    ohkeys = hkeys + hslots;
+    hcounts = reinterpret_cast<uint32_t*>(ohkeys + hslots);
+    ohcounts = hcounts + hslots;
+    info = ohcounts + hslots;
+  }
+};
+}  // namespace
+}  // namespace cfb
+
+extern "C" int64_t cfb_region_graph_hist_workspace(int64_t table_slots) {
+  if (table_slots <= 0) return 0;
+  return table_slots * (2 * 8 + 3 * 4) + 4 + kHistSlotsPerSlot * table_slots * (2 * 8 + 2 * 4) + 8 * (int64_t)sizeof(uint32_t);
+}
+
+extern "C" int cfb_region_graph_hist_device(const float* d_affs, int32_t flip_channel, const uint32_t* d_fragments, int64_t z, int64_t y,
+                                            int64_t x, int32_t bins, void* d_workspace, int64_t table_slots, int64_t* num_edges,
+                                            int64_t* num_entries, void* stream) {
+  return guarded([&]() -> int {
+    if (!d_affs || !d_fragments || !d_workspace || !num_edges || !num_entries) throw std::invalid_argument("region graph: null argument");
+    if (table_slots < 2 || (table_slots & (table_slots - 1)) || table_slots >= ((int64_t)1 << 31))
+      throw std::invalid_argument("region graph: table_slots must be a power of two below 2^31");
+    if (bins < 2 || bins > 256) throw std::invalid_argument("region graph: bins must be in 2..256");
+    const WsGeom g = ws_geom(z, y, x);
+    cudaStream_t s = (cudaStream_t)stream;
+    HistWorkspace w(d_workspace, table_slots);
+    CFB_CUDA(cudaMemsetAsync(w.keys, 0, (size_t)table_slots * 8, s));
+    CFB_CUDA(cudaMemsetAsync(w.maxbits, 0, (size_t)table_slots * 4, s));
+    CFB_CUDA(cudaMemsetAsync(w.hkeys, 0, (size_t)w.hslots * 8, s));
+    CFB_CUDA(cudaMemsetAsync(w.hcounts, 0, (size_t)w.hslots * 4, s));
+    CFB_CUDA(cudaMemsetAsync(w.info, 0, 8 * sizeof(uint32_t), s));
+    const int flip = flip_channel ? 1 : 0;
+    launch(rg_accumulate_kernel<true>, grid_for(g.n), kT, 0, s, d_affs, d_fragments, g, flip, w.keys, (unsigned long long*)nullptr,
+           (uint32_t*)nullptr, w.maxbits, (unsigned long long)(table_slots - 1), w.info);
+    launch(rg_hist_kernel, grid_for(g.n), kT, 0, s, d_affs, d_fragments, g, flip, (const unsigned long long*)w.keys,
+           (unsigned long long)(table_slots - 1), (int)bins, w.hkeys, w.hcounts, (unsigned long long)(w.hslots - 1), w.info);
+    uint32_t h_info[4] = {0, 0, 0, 0};
+    CFB_CUDA(cudaMemcpyAsync(h_info, w.info, sizeof(h_info), cudaMemcpyDeviceToHost, s));
+    CFB_CUDA(cudaStreamSynchronize(s));
+    *num_edges = h_info[0];
+    *num_entries = h_info[2];
+    if (h_info[1] || h_info[3]) {
+      set_last_error("region graph: the hash table is too small for this many fragment pairs or histogram bins");
+      return CFB_ERR_CAPACITY;
+    }
+    return CFB_OK;
+  });
+}
+
+extern "C" int cfb_region_graph_hist_read(void* d_workspace, int64_t table_slots, int64_t num_edges, int64_t num_entries, uint32_t* h_u,
+                                          uint32_t* h_v, uint64_t* h_offsets, uint8_t* h_bins, uint32_t* h_counts, float* h_max,
+                                          void* stream) {
+  return guarded([&]() -> int {
+    if (!d_workspace || table_slots < 2 || num_edges < 0 || num_edges > table_slots || num_entries < num_edges ||
+        num_entries > kHistSlotsPerSlot * table_slots)
+      throw std::invalid_argument("region graph read: bad argument");
+    if (!h_offsets) throw std::invalid_argument("region graph read: null output");
+    h_offsets[0] = 0;
+    if (num_edges == 0) return CFB_OK;
+    if (!h_u || !h_v || !h_bins || !h_counts || !h_max) throw std::invalid_argument("region graph read: null output");
+    cudaStream_t s = (cudaStream_t)stream;
+    HistWorkspace w(d_workspace, table_slots);
+    CFB_CUDA(cudaMemsetAsync(w.info + 4, 0, 2 * sizeof(uint32_t), s));
+    launch(rg_hist_gather_pairs_kernel, grid_for(table_slots), kT, 0, s, (const unsigned long long*)w.keys, (const uint32_t*)w.maxbits,
+           table_slots, w.okeys, w.omax, w.slot_index, w.info + 4);
+    launch(rg_hist_gather_bins_kernel, grid_for(w.hslots), kT, 0, s, (const unsigned long long*)w.hkeys, (const uint32_t*)w.hcounts,
+           w.hslots, (const uint32_t*)w.slot_index, w.ohkeys, w.ohcounts, w.info + 5);
+    std::vector<unsigned long long> k((size_t)num_edges), hk((size_t)num_entries);
+    std::vector<uint32_t> mx((size_t)num_edges), hc((size_t)num_entries);
+    uint32_t got[2] = {0, 0};
+    CFB_CUDA(cudaMemcpyAsync(got, w.info + 4, sizeof(got), cudaMemcpyDeviceToHost, s));
+    CFB_CUDA(cudaMemcpyAsync(k.data(), w.okeys, (size_t)num_edges * 8, cudaMemcpyDeviceToHost, s));
+    CFB_CUDA(cudaMemcpyAsync(mx.data(), w.omax, (size_t)num_edges * 4, cudaMemcpyDeviceToHost, s));
+    CFB_CUDA(cudaMemcpyAsync(hk.data(), w.ohkeys, (size_t)num_entries * 8, cudaMemcpyDeviceToHost, s));
+    CFB_CUDA(cudaMemcpyAsync(hc.data(), w.ohcounts, (size_t)num_entries * 4, cudaMemcpyDeviceToHost, s));
+    CFB_CUDA(cudaStreamSynchronize(s));
+    if ((int64_t)got[0] != num_edges || (int64_t)got[1] != num_entries)
+      throw std::invalid_argument("region graph read: num_edges or num_entries does not match the tables");
+    std::vector<uint32_t> order, rank((size_t)num_edges);
+    sorted_edge_order(k.data(), k.size(), order);   // the gather order is arbitrary
+    for (size_t i = 0; i < order.size(); ++i) {
+      const uint32_t o = order[i];
+      rank[o] = (uint32_t)i;
+      h_u[i] = (uint32_t)(k[o] >> 32);
+      h_v[i] = (uint32_t)(k[o] & 0xFFFFFFFFULL);
+      std::memcpy(&h_max[i], &mx[o], 4);
+      h_offsets[i + 1] = 0;
+    }
+    for (const unsigned long long e : hk) ++h_offsets[rank[e >> 8] + 1];   // CSR by sorted edge, then each run sorted by bin
+    for (int64_t i = 0; i < num_edges; ++i) h_offsets[i + 1] += h_offsets[i];
+    std::vector<uint64_t> cursor(h_offsets, h_offsets + num_edges);
+    for (size_t j = 0; j < hk.size(); ++j) {
+      const uint64_t p = cursor[rank[hk[j] >> 8]]++;
+      h_bins[p] = (uint8_t)(hk[j] & 0xFF);
+      h_counts[p] = hc[j];
+    }
+    for (int64_t i = 0; i < num_edges; ++i)
+      for (uint64_t p = h_offsets[i] + 1; p < h_offsets[i + 1]; ++p)   // insertion sort: a run holds at most 256 bins
+        for (uint64_t q = p; q > h_offsets[i] && h_bins[q - 1] > h_bins[q]; --q) {
+          std::swap(h_bins[q - 1], h_bins[q]);
+          std::swap(h_counts[q - 1], h_counts[q]);
+        }
     return CFB_OK;
   });
 }

@@ -144,10 +144,18 @@ __device__ __forceinline__ long long rg_quantize(float a) {
   return __double2ll_rn(v * 1073741824.0);
 }
 
+// an affinity clamped to [0, 1] in float32, NaN (and -0) as +0: the value rg_quantize quantises
+__device__ __forceinline__ float rg_clamp(float a) { return a > 0.f ? fminf(a, 1.f) : 0.f; }
+
+// kHist = false: the mean's statistics (sums, counts).  kHist = true: the first pass of the histogram region graph -- the
+// same pair table, with the largest clamped face affinity per pair instead (atomicMax on the float bits: all values are
+// >= +0, whose bit patterns order like the floats); `sums` and `counts` are unused and `maxbits` is written.
+template <bool kHist>
 __global__ void __launch_bounds__(kT) rg_accumulate_kernel(const float* __restrict__ affs, const uint32_t* __restrict__ frag, WsGeom g,
                                                            int flip, unsigned long long* __restrict__ keys,
                                                            unsigned long long* __restrict__ sums, uint32_t* __restrict__ counts,
-                                                           unsigned long long mask, uint32_t* __restrict__ info) {
+                                                           uint32_t* __restrict__ maxbits, unsigned long long mask,
+                                                           uint32_t* __restrict__ info) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < g.n; i += (int64_t)gridDim.x * blockDim.x) {
     const uint32_t id1 = frag[i];
     if (!id1) continue;
@@ -159,7 +167,8 @@ __global__ void __launch_bounds__(kT) rg_accumulate_kernel(const float* __restri
       const uint32_t id2 = frag[i - g.step[a]];
       if (!id2 || id2 == id1) continue;
       const unsigned long long key = ((unsigned long long)min(id1, id2) << 32) | max(id1, id2);
-      const long long q = rg_quantize(affs[(int64_t)(flip ? 2 - a : a) * g.n + i]);
+      const float aff = affs[(int64_t)(flip ? 2 - a : a) * g.n + i];
+      const long long q = rg_quantize(aff);   // (unused, and dropped, with kHist)
       unsigned long long h = rg_hash(key) & mask;
       bool done = false;
       for (int probe = 0; probe < kRgMaxProbe; ++probe, h = (h + 1) & mask) {
@@ -170,8 +179,15 @@ __global__ void __launch_bounds__(kT) rg_accumulate_kernel(const float* __restri
           if (cur == 0ULL) atomicAdd(&info[0], 1u);
           else if (cur != key) continue;
         }
-        atomicAdd(&sums[h], (unsigned long long)q);
-        atomicAdd(&counts[h], 1u);
+        if constexpr (kHist) {
+          const float c = rg_clamp(aff);
+          uint32_t bits;
+          memcpy(&bits, &c, sizeof bits);
+          atomicMax(&maxbits[h], bits);
+        } else {
+          atomicAdd(&sums[h], (unsigned long long)q);
+          atomicAdd(&counts[h], 1u);
+        }
         done = true;
         break;
       }
@@ -189,6 +205,80 @@ __global__ void __launch_bounds__(kT) rg_gather_kernel(const unsigned long long*
     if (!k) continue;
     const uint32_t o = atomicAdd(cursor, 1u);
     okeys[o] = k; osums[o] = sums[i]; ocounts[o] = counts[i];
+  }
+}
+
+// ---- histogram region graph (waterz HistogramQuantileAffinity): per pair of fragments, the number of faces whose clamped
+// affinity falls in each of `bins` bins, bin = min((int)(a * bins), bins - 1) in float32.  Second pass over the faces, after
+// rg_accumulate_kernel<true> built the pair table: every face finds its pair's slot and counts into a second table keyed by
+// ((slot + 1) << 8 | bin) (never 0: slots are below 2^31 and bins below 256).  info[2] = entries, info[3] = overflow.
+__global__ void __launch_bounds__(kT) rg_hist_kernel(const float* __restrict__ affs, const uint32_t* __restrict__ frag, WsGeom g, int flip,
+                                                     const unsigned long long* __restrict__ keys, unsigned long long mask, int bins,
+                                                     unsigned long long* __restrict__ hkeys, uint32_t* __restrict__ hcounts,
+                                                     unsigned long long hmask, uint32_t* __restrict__ info) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < g.n; i += (int64_t)gridDim.x * blockDim.x) {
+    const uint32_t id1 = frag[i];
+    if (!id1) continue;
+    int c[3];
+    ws_coords(i, g.sz, c);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      if (c[a] == 0) continue;
+      const uint32_t id2 = frag[i - g.step[a]];
+      if (!id2 || id2 == id1) continue;
+      const unsigned long long key = ((unsigned long long)min(id1, id2) << 32) | max(id1, id2);
+      unsigned long long h = rg_hash(key) & mask;
+      int probe = 0;
+      for (; probe < kRgMaxProbe && keys[h] != key; ++probe) {
+        if (keys[h] == 0ULL) { probe = kRgMaxProbe; break; }   // not in the table: the first pass overflowed and says so
+        h = (h + 1) & mask;
+      }
+      if (probe == kRgMaxProbe) continue;
+      const int bin = min((int)__fmul_rn(rg_clamp(affs[(int64_t)(flip ? 2 - a : a) * g.n + i]), (float)bins), bins - 1);
+      const unsigned long long hkey = ((h + 1ULL) << 8) | (unsigned long long)bin;
+      unsigned long long s = rg_hash(hkey) & hmask;
+      bool done = false;
+      for (int p = 0; p < kRgMaxProbe; ++p, s = (s + 1) & hmask) {
+        unsigned long long cur = *reinterpret_cast<volatile unsigned long long*>(hkeys + s);
+        if (cur != hkey) {
+          if (cur != 0ULL) continue;
+          cur = atomicCAS(&hkeys[s], 0ULL, hkey);
+          if (cur == 0ULL) atomicAdd(&info[2], 1u);
+          else if (cur != hkey) continue;
+        }
+        atomicAdd(&hcounts[s], 1u);
+        done = true;
+        break;
+      }
+      if (!done) info[3] = 1u;
+    }
+  }
+}
+
+// compaction of the pair table: (key, max) per pair in arbitrary order, and slot_index[slot] = its position
+__global__ void __launch_bounds__(kT) rg_hist_gather_pairs_kernel(const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ maxbits,
+                                                                  int64_t slots, unsigned long long* __restrict__ okeys,
+                                                                  uint32_t* __restrict__ omax, uint32_t* __restrict__ slot_index,
+                                                                  uint32_t* __restrict__ cursor) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < slots; i += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned long long k = keys[i];
+    if (!k) continue;
+    const uint32_t o = atomicAdd(cursor, 1u);
+    okeys[o] = k; omax[o] = maxbits[i]; slot_index[i] = o;
+  }
+}
+
+// compaction of the bin table: (pair position << 8 | bin, count), arbitrary order
+__global__ void __launch_bounds__(kT) rg_hist_gather_bins_kernel(const unsigned long long* __restrict__ hkeys, const uint32_t* __restrict__ hcounts,
+                                                                 int64_t hslots, const uint32_t* __restrict__ slot_index,
+                                                                 unsigned long long* __restrict__ okeys, uint32_t* __restrict__ ocounts,
+                                                                 uint32_t* __restrict__ cursor) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < hslots; i += (int64_t)gridDim.x * blockDim.x) {
+    const unsigned long long k = hkeys[i];
+    if (!k) continue;
+    const uint32_t o = atomicAdd(cursor, 1u);
+    okeys[o] = ((unsigned long long)slot_index[(k >> 8) - 1] << 8) | (k & 0xFFULL);
+    ocounts[o] = hcounts[i];
   }
 }
 

@@ -279,22 +279,28 @@ def connected_components(tasks, name, input_chunk_name, output_chunk_name, thres
 @click.option("--name", type=str, default="agglomerate", help="name of this operator")
 @click.option("--input-chunk-name", "-i", type=str, default="chunk", help="input chunk name (the affinity map)")
 @click.option("--output-chunk-name", "-o", type=str, default="chunk", help="output chunk name (the segmentation)")
-@click.option("--threshold", "-t", type=click.FLOAT, default=0.7, help="merge until the score 1 - mean affinity reaches this.")
+@click.option("--threshold", "-t", type=click.FLOAT, default=0.7, help="merge until the score (1 - mean affinity by default) reaches this.")
 @click.option("--aff-threshold-low", type=click.FLOAT, default=0.001, help="watershed: affinities up to this are no edges.")
 @click.option("--aff-threshold-high", type=click.FLOAT, default=0.9999, help="watershed: affinities from this on always connect.")
 @click.option("--flip-channel/--no-flip-channel", default=True,
               help="the channels are stored x, y, z (chunkflow) and read in reverse (waterz wants z, y, x).")
+@click.option("--scoring-function", type=str, default='OneMinus<MeanAffinity<RegionGraphType, ScoreValue>>',
+              help="waterz's scoring function: the mean affinity, or "
+                   "'OneMinus<HistogramQuantileAffinity<RegionGraphType, Q, ScoreValue, B[, I]>>'.")
 @operator
-def agglomerate(tasks, name, input_chunk_name, output_chunk_name, threshold, aff_threshold_low, aff_threshold_high, flip_channel):
-    """Watershed + mean-affinity agglomeration of an affinity map (the reference runs this as `plugin -f agglomerate`:
+def agglomerate(tasks, name, input_chunk_name, output_chunk_name, threshold, aff_threshold_low, aff_threshold_high, flip_channel,
+                scoring_function):
+    """Watershed + agglomeration of an affinity map (the reference runs this as `plugin -f agglomerate`:
     plugins/agglomerate.py:8-48 -> waterz.agglomerate; README.md:39)."""
+    from chunkflow_b200.chunk.device import parse_scoring_function
+    parse_scoring_function(scoring_function)
     import torch
     for task in tasks:
         if task is not None:
             start = time()
             dev, was_host = _on_device(task[input_chunk_name], "cuda:0")
             out = dev.agglomerate(threshold=threshold, aff_threshold_low=aff_threshold_low, aff_threshold_high=aff_threshold_high,
-                                  flip_channel=flip_channel)
+                                  flip_channel=flip_channel, scoring_function=scoring_function)
             torch.cuda.synchronize(out.tensor.device)
             task[output_chunk_name] = out.to_chunk() if was_host else out
             task["log"]["timer"][name] = time() - start

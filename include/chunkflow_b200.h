@@ -305,6 +305,31 @@ int cfb_region_graph_read(void* d_workspace, int64_t table_slots, int64_t num_ed
 int cfb_agglomerate_edges_host(int64_t num_nodes, int64_t num_edges, const uint32_t* u, const uint32_t* v,
                                const uint64_t* sum_fixed, const uint32_t* count, float threshold, uint32_t* root_of);
 
+/* Histogram region graph (waterz's HistogramQuantileAffinity statistics): for every pair of touching fragments (the faces
+ * and channels of cfb_region_graph_device) the number of faces whose affinity a -- clamped to [0,1], NaN = 0, float32 --
+ * falls in bin min((int)(a * bins), bins - 1), 2 <= bins <= 256, and the largest clamped affinity.  Two passes over the
+ * faces: the pair table, then a table of (pair, bin) counts of 2 x table_slots slots, both inside d_workspace
+ * (cfb_region_graph_hist_workspace(table_slots) bytes); CFB_ERR_CAPACITY when either is too full -- call again with more slots.
+ * *num_edges = pairs, *num_entries = non-empty (pair, bin) counts.  cfb_region_graph_hist_read copies them to the host:
+ * edges sorted by (u, v), u < v, with their maxima; h_offsets (num_edges + 1) delimits each edge's run of h_bins / h_counts,
+ * sorted by bin. */
+int64_t cfb_region_graph_hist_workspace(int64_t table_slots);
+int cfb_region_graph_hist_device(const float* d_affs, int32_t flip_channel, const uint32_t* d_fragments, int64_t z, int64_t y,
+                                 int64_t x, int32_t bins, void* d_workspace, int64_t table_slots, int64_t* num_edges,
+                                 int64_t* num_entries, void* stream);
+int cfb_region_graph_hist_read(void* d_workspace, int64_t table_slots, int64_t num_edges, int64_t num_entries, uint32_t* h_u,
+                               uint32_t* h_v, uint64_t* h_offsets, uint8_t* h_bins, uint32_t* h_counts, float* h_max, void* stream);
+
+/* The merge loop with OneMinus<HistogramQuantileAffinity<RegionGraphType, quantile, ScoreValue, num_bins, init_with_max>>,
+ * on the host.  Edge i holds the bins offsets[i] .. offsets[i+1] (strictly increasing, < num_bins, non-zero counts) and, when
+ * init_with_max, maxima[i] in [0, 1] (maxima may be NULL otherwise).  score = 1 - (q + 0.5) / num_bins, q the first bin whose
+ * cumulative count reaches min(floor(quantile * n / 100) + 1, n) of the n faces; with init_with_max, an edge that has never
+ * been pooled scores 1 - its maximum.  Pooled edges add their histograms and keep the anchor of the one that comes first in
+ * (score, anchor) order.  Otherwise as cfb_agglomerate_edges_host (rules: oracle/agglomeration_oracle.py). */
+int cfb_agglomerate_quantile_host(int64_t num_nodes, int64_t num_edges, const uint32_t* u, const uint32_t* v, const uint64_t* offsets,
+                                  const uint8_t* bins, const uint32_t* counts, const float* maxima, int32_t quantile,
+                                  int32_t num_bins, int32_t init_with_max, float threshold, uint32_t* root_of);
+
 /* d_out[i] = d_map[d_labels[i]] (labels >= map_size pass through): applies root_of to the fragments. */
 int cfb_relabel_device(const uint32_t* d_labels, int64_t n, const uint32_t* d_map, int64_t map_size, uint32_t* d_out,
                        void* stream);
