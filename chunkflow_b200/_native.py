@@ -39,6 +39,7 @@ EXPORTS = (
     "cfb_label_apply_device", "cfb_downsample_average_device", "cfb_downsample_workspace", "cfb_downsample_segmentation_device",
     "cfb_gaussian_filter_workspace", "cfb_gaussian_filter_device", "cfb_median_filter_device",
     "cfb_clahe_workspace", "cfb_clahe_device",
+    "cfb_mesh_workspace", "cfb_mesh_count_device", "cfb_mesh_buffer_bytes", "cfb_mesh_device", "cfb_mesh_read", "cfb_mesh_simplify_host",
 )
 
 
@@ -175,6 +176,7 @@ def load() -> C.CDLL:
     lib.cfb_median_filter_device.argtypes = [vp, i32, i64, i64, i64, i64, C.POINTER(i64 * 4), i32, vp, vp]
     lib.cfb_clahe_workspace.argtypes = [i64, i64, i64, i32, i32, C.POINTER(i64)]
     lib.cfb_clahe_device.argtypes = [vp, vp, i64, i64, i64, C.c_double, i32, i32, vp, i64, vp]
+    bind_mesh(lib)
     for name in EXPORTS:
         getattr(lib, name)   # every declared symbol must be there
     _lib = lib
@@ -599,6 +601,99 @@ def clahe_device(d_in: int, d_out: int, shape, clip_limit: float, tile_grid_size
     zyx, tx, ty = clahe_args(shape, tile_grid_size)
     check(load().cfb_clahe_device(C.c_void_p(d_in), C.c_void_p(d_out), *zyx, float(clip_limit), tx, ty,
                                   C.c_void_p(d_workspace or None), int(workspace_bytes), C.c_void_p(stream)))
+
+
+# ---- `mesh` (include/chunkflow_b200.h) ----
+MESH_DTYPES = (DTYPE_U32, DTYPE_U64)
+
+
+def bind_mesh(lib: C.CDLL) -> None:
+    """Argument types of the mesh entry points (also for the host emulation of csrc/mesh.cu)."""
+    vp, i32, i64, pi64 = C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_int64)
+    lib.cfb_mesh_workspace.argtypes = [i64, i64, i64, i32, pi64]
+    lib.cfb_mesh_count_device.argtypes = [vp, i32, i64, i64, i64, vp, i64, i32, vp, pi64, pi64, pi64, vp]
+    lib.cfb_mesh_buffer_bytes.argtypes = [i64, i64, i64, pi64]
+    lib.cfb_mesh_device.argtypes = [vp, i32, i64, i64, i64, vp, i64, i32, vp, vp, i64, i64, i64, vp, i64, pi64, vp]
+    lib.cfb_mesh_read.argtypes = [vp, i64, i64, i64, i64, vp, vp, vp, vp, vp, vp]
+    lib.cfb_mesh_simplify_host.argtypes = [i64, vp, i64, vp, i64, C.c_double, pi64, vp, pi64, vp]
+
+
+def _mesh_dtype(dtype) -> int:
+    if dtype not in MESH_DTYPES:
+        raise TypeError("a segmentation to mesh is DTYPE_U32 or DTYPE_U64")
+    return int(dtype)
+
+
+def mesh_workspace(zyx, close: bool, lib=None) -> int:
+    """Bytes of the count workspace of a (z, y, x) volume (no device needed)."""
+    lib, out = lib or load(), C.c_int64()
+    _mesh_check(lib, lib.cfb_mesh_workspace(*(int(v) for v in zyx), int(bool(close)), C.byref(out)))
+    return int(out.value)
+
+
+def mesh_count_device(d_labels: int, dtype: int, zyx, d_skip: int, num_skip: int, close: bool, d_workspace: int, stream: int = 0,
+                      lib=None):
+    """-> ((cube, object) pairs, triangles, vertices) of the segmentation at ``d_labels`` (synchronises the stream)."""
+    pairs, tris, verts = C.c_int64(), C.c_int64(), C.c_int64()
+    lib = lib or load()
+    _mesh_check(lib, lib.cfb_mesh_count_device(C.c_void_p(d_labels), _mesh_dtype(dtype), *(int(v) for v in zyx), C.c_void_p(d_skip or None),
+                                               int(num_skip), int(bool(close)), C.c_void_p(d_workspace), C.byref(pairs), C.byref(tris),
+                                               C.byref(verts), C.c_void_p(stream)))
+    return int(pairs.value), int(tris.value), int(verts.value)
+
+
+def mesh_buffer_bytes(counts, lib=None) -> int:
+    """Bytes of the device buffer of the weld for the counts of mesh_count_device (no device needed)."""
+    lib, out = lib or load(), C.c_int64()
+    pairs, tris, verts = (int(v) for v in counts)
+    _mesh_check(lib, lib.cfb_mesh_buffer_bytes(pairs, tris, verts, C.byref(out)))
+    return int(out.value)
+
+
+def mesh_device(d_labels: int, dtype: int, zyx, d_skip: int, num_skip: int, close: bool, voxel_size, d_workspace: int, counts,
+                d_buffer: int, buffer_bytes: int, stream: int = 0, lib=None) -> int:
+    """Every mesh welded on the device into ``d_buffer`` -> the number of objects (synchronises the stream)."""
+    vs = np.ascontiguousarray(voxel_size, np.float64)
+    if vs.shape != (3,):
+        raise ValueError("the voxel size is (z, y, x)")
+    pairs, tris, verts = (int(v) for v in counts)
+    n, lib = C.c_int64(), lib or load()
+    _mesh_check(lib, lib.cfb_mesh_device(C.c_void_p(d_labels), _mesh_dtype(dtype), *(int(v) for v in zyx), C.c_void_p(d_skip or None),
+                                         int(num_skip), int(bool(close)), _ptr(vs), C.c_void_p(d_workspace), pairs, tris, verts,
+                                         C.c_void_p(d_buffer), int(buffer_bytes), C.byref(n), C.c_void_p(stream)))
+    return int(n.value)
+
+
+def mesh_read(d_buffer: int, counts, num_objects: int, stream: int = 0, lib=None) -> dict:
+    """The meshes of mesh_device -> {id: (vertices float32 (N, 3) xyz, faces uint32 (M, 3))}, ids ascending."""
+    pairs, tris, verts = (int(v) for v in counts)
+    n = int(num_objects)
+    obj, fo, vo = np.empty(n, np.uint64), np.empty(n + 1, np.int64), np.empty(n + 1, np.int64)
+    faces, vertices = np.empty((tris, 3), np.uint32), np.empty((verts, 3), np.float32)
+    lib = lib or load()
+    _mesh_check(lib, lib.cfb_mesh_read(C.c_void_p(d_buffer), pairs, tris, verts, n, _ptr(obj), _ptr(fo), _ptr(vo), _ptr(faces),
+                                       _ptr(vertices), C.c_void_p(stream)))
+    return {int(obj[o]): (vertices[vo[o]:vo[o + 1]], faces[fo[o]:fo[o + 1]]) for o in range(n)}
+
+
+def mesh_simplify_host(vertices, faces, simplification_factor: int, max_simplification_error: float, lib=None):
+    """One mesh simplified on the host (no GPU involved) -> (vertices float32 (N, 3), faces uint32 (M, 3))."""
+    v, f = np.ascontiguousarray(vertices, np.float32), np.ascontiguousarray(faces, np.uint32)
+    if v.ndim != 2 or v.shape[1] != 3 or f.ndim != 2 or f.shape[1] != 3:
+        raise ValueError("vertices (N, 3) and faces (M, 3)")
+    if isinstance(simplification_factor, bool) or not isinstance(simplification_factor, (int, np.integer)):
+        raise TypeError("the simplification factor is an integer")
+    ov, of = np.empty_like(v), np.empty_like(f)
+    nv, nf = C.c_int64(), C.c_int64()
+    lib = lib or load()
+    _mesh_check(lib, lib.cfb_mesh_simplify_host(v.shape[0], _ptr(v), f.shape[0], _ptr(f), int(simplification_factor),
+                                                float(max_simplification_error), C.byref(nv), _ptr(ov), C.byref(nf), _ptr(of)))
+    return ov[:nv.value].copy(), of[:nf.value].copy()
+
+
+def _mesh_check(lib, code: int) -> None:
+    if code != OK:
+        raise NativeError(code, lib.cfb_last_error().decode("utf-8", "replace"))
 
 
 def device_memory(device: int = 0) -> tuple:

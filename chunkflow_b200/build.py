@@ -15,9 +15,12 @@ CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "_native")
 LIB_PATH = os.path.join(OUT_DIR, "libchunkflow_b200.so")
 
+# -ffp-contract=off for the host compiler, for every file on purpose: the host code computes what oracle/ restates and what the
+# host emulations (tests/host_emulation, built with the same flag) compute, every multiply and add rounded on its own, on any
+# host architecture (an FMA-capable host such as aarch64 would otherwise fuse them).
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
-    "-Xcompiler", "-fPIC", "-shared",
+    "-Xcompiler", "-fPIC", "-Xcompiler", "-ffp-contract=off", "-shared",
 ]
 
 

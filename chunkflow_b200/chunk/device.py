@@ -17,6 +17,7 @@ bookkeeping of the reference's ``Chunk`` and mirrors, name for name, the referen
     gaussian_filter_2d   reference chunk/base.py:846-853                (Chunk -> scipy.ndimage.gaussian_filter)
     median_filter        reference plugins/median_filter.py:4-7         (plugin -> scipy.ndimage.median_filter)
     clahe                reference plugins/clahe.py                     (plugin -> cv2.createCLAHE(...).apply)
+    mesh                 reference flow/mesh.py                         (MeshOperator -> zmesh; rules restated)
 
 so that ``create-chunk | normalize-contrast | inference | crop-margin | quantize`` moves the image to the GPU once and
 brings a uint8 thumbnail (or nothing) back instead of the 12-byte-per-voxel affinity map.  There is no CPU fallback.
@@ -698,6 +699,59 @@ class DeviceChunk:
                                  work_bytes, self._stream())
             del work   # the caching allocator keeps it for the stream until the kernels have run
         return DeviceChunk(out, voxel_offset=self.voxel_offset, voxel_size=self.voxel_size, layer_type=self.layer_type)
+
+    # ---- `mesh`: marching cubes on the device, welding and simplification on the host --------------------------------------
+    def mesh(self, voxel_size=None, simplification_factor: int = 100, max_simplification_error: float = 40, skip_ids=None,
+             close: bool = False, threads: int = 0) -> dict:
+        """Meshes of every object of a (z,y,x) segmentation (csrc/mesh.cu, rules in oracle/mesh_oracle.py; not zmesh's meshes):
+        ``{id: (vertices float32 (N, 3) x, y, z in physical units, faces uint32 (M, 3))}`` in the chunk's own frame, ids
+        ascending.  ``voxel_size`` is (z, y, x), the chunk's by default.  0 and the ``skip_ids`` are not meshed.  The mesh is
+        open at the chunk faces unless ``close`` (everything outside the chunk is then 0 and every object watertight).
+        ``simplification_factor`` > 1 simplifies each object towards ceil(faces / factor) faces while the error stays within
+        ``max_simplification_error`` (nm, like zmesh's).  uint32 / int32 / uint64 / int64 ids (signed ones by their bit
+        pattern); another dtype raises TypeError and another ndim ValueError before any kernel runs.  The meshes are welded on
+        the device; ``threads``: host workers of the simplifier (0: the hardware's); the result does not depend on it."""
+        torch = _torch()
+        t = self.tensor.contiguous()
+        if t.ndim != 3:
+            raise ValueError(f"mesh takes a (z, y, x) segmentation, not a {t.ndim}-D chunk")
+        codes = {torch.int32: _native.DTYPE_U32, torch.int64: _native.DTYPE_U64}
+        for name, code in (("uint32", _native.DTYPE_U32), ("uint64", _native.DTYPE_U64)):
+            if hasattr(torch, name):
+                codes[getattr(torch, name)] = code
+        if t.dtype not in codes:
+            raise TypeError(f"mesh takes uint32, int32, uint64 or int64 ids, not {t.dtype}")
+        if isinstance(simplification_factor, bool) or not isinstance(simplification_factor, (int, np.integer)):
+            raise TypeError("the simplification factor is an integer")
+        vs = self.voxel_size if voxel_size is None else voxel_size
+        vs = tuple(float(v) for v in (vs if vs is not None else (1, 1, 1)))
+        if len(vs) != 3:
+            raise ValueError(f"the voxel size is (z, y, x), not {vs}")
+        code = codes[t.dtype]
+        skip = selected_ids(skip_ids) if skip_ids is not None else np.zeros(0, np.uint64)
+        skip = np.unique(skip)
+        zyx = tuple(t.shape)
+        if min(zyx) == 0:
+            return {}
+        with self._on_device():
+            d_skip = torch.from_numpy(skip.view(np.int64)).to(t.device) if skip.size else None
+            work = torch.empty(_native.mesh_workspace(zyx, close), dtype=torch.uint8, device=t.device)
+            args = (t.data_ptr(), code, zyx, d_skip.data_ptr() if d_skip is not None else 0, skip.size, close)
+            counts = _native.mesh_count_device(*args, work.data_ptr(), self._stream())
+            nbytes = _native.mesh_buffer_bytes(counts)
+            buf = torch.empty(nbytes, dtype=torch.uint8, device=t.device)
+            n = _native.mesh_device(*args, vs, work.data_ptr(), counts, buf.data_ptr(), nbytes, self._stream())
+            meshes = _native.mesh_read(buf.data_ptr(), counts, n, self._stream())
+            del buf, work
+        if simplification_factor <= 1 or not meshes:
+            return meshes
+        from concurrent.futures import ThreadPoolExecutor   # the native simplifier releases the GIL
+        import os
+        workers = threads if threads > 0 else min(32, os.cpu_count() or 1)
+        keys = list(meshes)
+        with ThreadPoolExecutor(max_workers=workers) as pool:
+            out = pool.map(lambda k: _native.mesh_simplify_host(*meshes[k], simplification_factor, max_simplification_error), keys)
+            return dict(zip(keys, out))
 
     def __repr__(self):
         return f"DeviceChunk(shape={self.shape}, dtype={self.dtype}, voxel_offset={tuple(self.voxel_offset)}, device={self.tensor.device})"

@@ -463,5 +463,48 @@ def remap_segmentation(tasks, input_chunk_name, output_chunk_name, base_id):
         yield task
 
 
+@main.command("mesh")
+@click.option("--name", type=str, default="mesh", help="name of operator")
+@click.option("--input-chunk-name", "-i", type=str, default="chunk", help="name of chunk needs to be meshed.")
+@click.option("--mip", "-m", type=click.INT, default=None, help="mip level of segmentation chunk.")
+@click.option("--voxel-size", "-v", type=click.INT, nargs=3, default=None, callback=default_none,
+              help="voxel size of the segmentation. zyx order.")
+@click.option("--output-path", "-o", type=str, default="file:///tmp/mesh/",
+              help="output path of meshes: a local directory or file:// URL. With the precomputed format, the mesh directory "
+                   "named in its info file.")
+@click.option("--output-format", "-t", type=click.Choice(["ply", "obj", "precomputed"]), default="precomputed",
+              help="output format, could be one of ply|obj|precomputed.")
+@click.option("--simplification-factor", "-f", type=click.INT, default=100, help="mesh simplification factor.")
+@click.option("--max-simplification-error", "-e", type=click.INT, default=40, help="max simplification error.")
+@click.option("--skip-ids", "-s", type=str, default=None, help="do not mesh for some specific ids.")
+@click.option("--manifest/--no-manifest", default=False, help="create manifest file or not.")
+@click.option("--shard/--no-shard", default=False, help="combine meshes as one file")
+@operator
+def mesh(tasks, name, input_chunk_name, mip, voxel_size, output_path, output_format, simplification_factor,
+         max_simplification_error, skip_ids, manifest, shard):
+    """Perform meshing for segmentation chunk (reference flow/flow.py:2087-2135, flow/mesh.py): marching cubes on the GPU,
+    welding and simplification on the host (rules restated: not zmesh's meshes).  A host chunk is uploaded for the call, a
+    GPU-resident one is meshed where it is."""
+    from chunkflow_b200.flow.mesh import MeshWriter
+    if mip is None:
+        mip = state["mip"]
+    if skip_ids is not None:
+        skip_ids = frozenset(map(int, skip_ids.split(",")))
+    writer = MeshWriter(output_path, output_format, mip=mip, voxel_size=voxel_size, max_simplification_error=max_simplification_error,
+                        manifest=manifest, shard=shard)
+    for task in tasks:
+        if task is not None:
+            start = time()
+            seg = task[input_chunk_name]
+            dev, _ = _on_device(seg, "cuda:0")
+            vs = writer.voxel_size if writer.voxel_size is not None else seg.voxel_size
+            # the shard holds every object (as in the reference); the fragments skip the ids when they are written
+            meshes = dev.mesh(voxel_size=vs, simplification_factor=simplification_factor,
+                              max_simplification_error=max_simplification_error, skip_ids=None if shard else skip_ids)
+            writer.write(meshes, seg.voxel_offset, seg.shape[-3:], skip_ids=skip_ids)
+            task["log"]["timer"][name] = time() - start
+        yield task
+
+
 if __name__ == "__main__":
     main()

@@ -517,6 +517,52 @@ int cfb_clahe_workspace(int64_t z, int64_t y, int64_t x, int32_t tiles_x, int32_
 int cfb_clahe_device(const void* d_in, void* d_out, int64_t z, int64_t y, int64_t x, double clip_limit, int32_t tiles_x,
                      int32_t tiles_y, void* d_workspace, int64_t workspace_bytes, void* stream);
 
+/* `mesh` (reference flow/flow.py:2087-2135, flow/mesh.py -> zmesh): marching cubes of every object of a (z, y, x) segmentation,
+ * restated in oracle/mesh_oracle.py (zmesh is not vendored: its meshes are not reproduced, parity unpinned).
+ *   cubes     one per 2 x 2 x 2 group of voxel centres: z < Z-1, y < Y-1, x < X-1 (open, close = 0), or from -1 to Z-1 along
+ *             every axis with everything outside the chunk 0 (close != 0: every object comes out watertight).  For every
+ *             distinct id L among a cube's corners that is neither 0 nor among the d_skip_ids, the case is the mask of the
+ *             corners equal to L (corner c at dz, dy, dx = c >> 2 & 1, c >> 1 & 1, c & 1); its triangles come from one
+ *             256-case table built face by face (oracle/mesh_oracle.py), counter-clockwise seen from outside L.
+ *   vertices  one per (object, cut edge): on the cut axis at (i + 1) * voxel size, on the others at (i + 0.5) * voxel size,
+ *             for the edge's lower voxel i; float32, columns x, y, z.  Numbered in ascending order of the edge key
+ *             ((z + 1) * (Y + 2) + (y + 1)) * (X + 2) + (x + 1)) * 3 + axis (0 x, 1 y, 2 z).  Faces in raster order of their
+ *             cube, then in table order.
+ * cfb_mesh_workspace  bytes of d_workspace (the counts) for a volume.  No device needed.
+ * cfb_mesh_count_device  the (cube, object) pairs with a non-empty case, their triangles and the vertices (synchronises the
+ *     stream).  dtype CFB_DTYPE_U32 or CFB_DTYPE_U64; d_skip_ids: num_skip ids on the device, ascending.  2^32 or more
+ *     triangles or vertices return CFB_ERR_INVALID_ARGUMENT.
+ * cfb_mesh_buffer_bytes  bytes of d_buffer for those counts.  No device needed.
+ * cfb_mesh_device  after the count, with the same arguments, the workspace it filled and its counts: every mesh, welded on the
+ *     device into d_buffer; *num_objects = the objects meshed.  voxel_size is (z, y, x).  Synchronises the stream.
+ * cfb_mesh_read  the meshes to the host, objects in ascending order of id: object o has the faces face_offsets[o] ..
+ *     face_offsets[o + 1] (rows of faces, indices into its own vertices) and the vertices vertex_offsets[o] ..
+ *     vertex_offsets[o + 1] (rows of vertices).  object_ids holds num_objects entries, the offsets num_objects + 1, faces
+ *     num_triangles rows and vertices num_vertices rows, the counts of cfb_mesh_count_device.
+ * cfb_mesh_simplify_host  a restated Garland-Heckbert edge collapse of one mesh, fully ordered (rules:
+ *     oracle/mesh_oracle.py simplify).  Face quadrics of the unit-normal planes, unweighted, in float64; the ends of an
+ *     edge used by one face only (an open border) are locked.  Candidates: every edge not locked at both ends, placed at its
+ *     locked end or at the first of (v_a, v_b, midpoint) with the least error, the error being the cost.  Collapsed in
+ *     ascending (cost, a, b) order with lazy re-evaluation, a < b surviving with the summed quadric and re-queueing the edges
+ *     of a and of its neighbours (so that a refused collapse is tried again once its surroundings change), unless that breaks the
+ *     link condition, flips or degenerates a face that stays, or repeats a face's vertex set.  Stops at
+ *     ceil(num_faces / simplification_factor) faces or when the cheapest cost exceeds max_simplification_error^2.  Faces
+ *     keep their order, vertices are renumbered in order of first use; out_vertices and out_faces have room for the input.
+ *     simplification_factor <= 1 copies the mesh unchanged.  No device needed. */
+int cfb_mesh_workspace(int64_t z, int64_t y, int64_t x, int32_t close, int64_t* workspace_bytes);
+int cfb_mesh_count_device(const void* d_labels, int32_t dtype, int64_t z, int64_t y, int64_t x, const uint64_t* d_skip_ids,
+                          int64_t num_skip, int32_t close, void* d_workspace, int64_t* num_pairs, int64_t* num_triangles,
+                          int64_t* num_vertices, void* stream);
+int cfb_mesh_buffer_bytes(int64_t num_pairs, int64_t num_triangles, int64_t num_vertices, int64_t* buffer_bytes);
+int cfb_mesh_device(const void* d_labels, int32_t dtype, int64_t z, int64_t y, int64_t x, const uint64_t* d_skip_ids, int64_t num_skip,
+                    int32_t close, const double* voxel_size, void* d_workspace, int64_t num_pairs, int64_t num_triangles,
+                    int64_t num_vertices, void* d_buffer, int64_t buffer_bytes, int64_t* num_objects, void* stream);
+int cfb_mesh_read(void* d_buffer, int64_t num_pairs, int64_t num_triangles, int64_t num_vertices, int64_t num_objects, uint64_t* object_ids,
+                  int64_t* face_offsets, int64_t* vertex_offsets, uint32_t* faces, float* vertices, void* stream);
+int cfb_mesh_simplify_host(int64_t num_vertices, const float* vertices, int64_t num_faces, const uint32_t* faces,
+                           int64_t simplification_factor, double max_simplification_error, int64_t* out_num_vertices,
+                           float* out_vertices, int64_t* out_num_faces, uint32_t* out_faces);
+
 #ifdef __cplusplus
 }
 #endif
