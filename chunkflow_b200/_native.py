@@ -16,6 +16,7 @@ OK = 0
 ERR_INVALID_ARGUMENT, ERR_CUDA, ERR_WEIGHTS, ERR_OUTPUT_RANGE, ERR_UNSUPPORTED, ERR_CAPACITY = -1, -2, -3, -4, -5, -6
 FRAMEWORK_UNET3L, FRAMEWORK_IDENTITY = 0, 1
 PRECISION_F32_SIMT, PRECISION_F16X3_UMMA, PRECISION_F16_UMMA, PRECISION_F16F8_UMMA = 0, 1, 2, 3
+LAYER_OPS = ("conv3", "conv3_pool", "convT", "maxpool", "first", "head_sigmoid", "head_blend", "conv3_head_blend", "round_trip")
 DTYPE_U8, DTYPE_F32, DTYPE_U32, DTYPE_U64, DTYPE_BOOL = 0, 1, 2, 3, 4
 AUGMENT_NONE, AUGMENT_REFERENCE, AUGMENT_SPATIAL = 0, 1, 2
 QUANTIZE_XY, QUANTIZE_Z = 0, 1
@@ -28,7 +29,7 @@ EXPORTS = (
     "cfb_infer_chunk_device", "cfb_infer_chunk_host", "cfb_infer_slab_device", "cfb_normalize_device",
     "cfb_slab_nonzero", "cfb_halo_add_device", "cfb_weight_volume_device",
     "cfb_patch_forward_host", "cfb_make_patch_mask", "cfb_plugin_begin", "cfb_plugin_extract", "cfb_plugin_blend",
-    "cfb_plugin_end", "cfb_last_timing", "cfb_set_profiling", "cfb_layer_timing", "cfb_debug_net_forward_host", "cfb_debug_conv3_host",
+    "cfb_plugin_end", "cfb_last_timing", "cfb_set_profiling", "cfb_layer_timing", "cfb_debug_net_forward_host", "cfb_debug_layer_host",
     "cfb_normalize_contrast_device", "cfb_maskout_device", "cfb_crop_margin_device", "cfb_quantize_device",
     "cfb_connected_components_device", "cfb_connected_components_workspace",
     "cfb_watershed_workspace", "cfb_watershed_device", "cfb_region_graph_workspace", "cfb_region_graph_device",
@@ -68,6 +69,20 @@ class SegScores(C.Structure):
 
     def as_dict(self) -> dict:
         return {name: getattr(self, name) for name, _ in self._fields_ if name not in ("struct_size", "reserved")}
+
+
+class LayerArgs(C.Structure):
+    """cfb_layer_args: one step of the U-Net layer table for cfb_debug_layer_host."""
+    _fields_ = [
+        ("struct_size", C.c_int32), ("op", C.c_int32), ("nb", C.c_int32), ("size", C.c_int32 * 3),
+        ("ca", C.c_int32), ("cb", C.c_int32), ("cout", C.c_int32), ("relu", C.c_int32),
+        ("a", C.c_void_p), ("b", C.c_void_p), ("weight", C.c_void_p), ("bias", C.c_void_p),
+        ("head_weight", C.c_void_p), ("head_bias", C.c_void_p), ("head_channels", C.c_int32),
+        ("chunk_dtype", C.c_int32), ("chunk", C.c_void_p), ("chunk_size", C.c_int32 * 3),
+        ("out_patch", C.c_int32 * 3), ("crop", C.c_int32 * 3), ("out_size", C.c_int32 * 3),
+        ("in_origins", C.c_void_p), ("out_origins", C.c_void_p), ("mask", C.c_void_p), ("scale", C.c_float),
+        ("out", C.c_void_p), ("pooled", C.c_void_p),
+    ]
 
 
 class NativeError(RuntimeError):
@@ -133,7 +148,7 @@ def load() -> C.CDLL:
     lib.cfb_set_profiling.argtypes = [vp, i32]
     lib.cfb_layer_timing.argtypes = [vp, i32, C.POINTER(i32), vp, vp, vp]
     lib.cfb_debug_net_forward_host.argtypes = [vp, vp, vp]
-    lib.cfb_debug_conv3_host.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, i32, i32, vp]
+    lib.cfb_debug_layer_host.argtypes = [vp, C.POINTER(LayerArgs)]
     lib.cfb_normalize_contrast_device.argtypes = [vp, i64, i64, i64, C.c_double, C.c_double, i32, i32, i32, vp]
     lib.cfb_maskout_device.argtypes = [vp, i32, i64, i64, i64, i64, vp, i32, i64, i64, i64, vp]
     lib.cfb_crop_margin_device.argtypes = [vp, i32, i64, i64, i64, i64, C.POINTER(i64 * 6), vp, vp]
@@ -902,9 +917,71 @@ class Engine:
         return out
 
     def debug_conv3(self, x: np.ndarray, w: np.ndarray, b: np.ndarray, relu: bool) -> np.ndarray:
-        x = np.ascontiguousarray(x, np.float32); w = np.ascontiguousarray(w, np.float32); b = np.ascontiguousarray(b, np.float32)
-        cin, z, y, xx = x.shape
-        cout = w.shape[0]
-        out = np.empty((cout, z, y, xx), np.float32)
-        check(self._lib.cfb_debug_conv3_host(self._h, _ptr(x), cin, z, y, xx, _ptr(w), _ptr(b), cout, int(relu), _ptr(out)))
-        return out
+        """One 3x3x3 convolution of one patch, x (cin, z, y, x) -> (cout, z, y, x), through debug_layer; for cin >= 32 the
+        input is fed as two sources of cin / 2 channels (the decoders' concat)."""
+        x = np.asarray(x, np.float32)[None]
+        cb = x.shape[1] // 2 if x.shape[1] >= 32 else 0
+        ca = x.shape[1] - cb
+        return self.debug_layer("conv3", x[:, :ca], x[:, ca:] if cb else None, w, b, relu=relu)[0]
+
+    def debug_layer(self, op: str, a: np.ndarray, b: Optional[np.ndarray] = None, weight=None, bias=None, relu: bool = True,
+                    head_weight=None, head_bias=None, chunk: Optional[np.ndarray] = None, in_origins=None, out_origins=None,
+                    out_patch=None, crop=(0, 0, 0), mask=None, out: Optional[np.ndarray] = None, scale: float = 1.0, size=None):
+        """One step of the layer table through the kernels of this engine's precision mode (cfb_debug_layer_host).
+
+        `op` is one of LAYER_OPS.  `a` (nb, ca, z, y, x) and `b` (nb, cb, z, y, x) are the two sources of a concat (`a` is
+        (nb, 1, z, y, x) for 'first', or None with `chunk`, `in_origins` (nb, 3) and the patch `size`).  Returns the output array, or (output, pooled)
+        for 'conv3_pool'; the blending ops accumulate into `out` (channels, *out_size) and return it."""
+        code = LAYER_OPS.index(op)
+        keep = []
+
+        def arr(v, dtype=np.float32):
+            if v is None:
+                return None
+            v = np.ascontiguousarray(v, dtype)
+            keep.append(v)
+            return v
+
+        def ptr(v):
+            return None if v is None else v.ctypes.data
+
+        chunk = None if chunk is None else np.ascontiguousarray(chunk)
+        a, b, weight, bias = arr(a), arr(b), arr(weight), arr(bias)
+        head_weight, head_bias, mask = arr(head_weight), arr(head_bias), arr(mask)
+        in_origins, out_origins = arr(in_origins, np.int32), arr(out_origins, np.int32)
+        if a is not None:
+            nb, ca, z, y, x = a.shape
+        else:
+            nb, ca, (z, y, x) = len(in_origins), 1, (int(v) for v in size)
+        cb = 0 if b is None else b.shape[1]
+        cout = {"conv3": None, "conv3_pool": None, "convT": None, "maxpool": ca, "first": 16, "head_sigmoid": None,
+                "head_blend": None, "conv3_head_blend": 16, "round_trip": ca}[op]
+        if cout is None:
+            cout = weight.shape[1] if op == "convT" else weight.shape[0] if weight is not None else 0
+        hc = 0 if head_weight is None else head_weight.shape[0]
+        p = LayerArgs()
+        p.struct_size = C.sizeof(LayerArgs)
+        p.op, p.nb, p.ca, p.cb, p.cout, p.relu = code, nb, ca, cb, cout, int(bool(relu))
+        p.size[:] = [z, y, x]
+        p.a, p.b, p.weight, p.bias = ptr(a), ptr(b), ptr(weight), ptr(bias)
+        p.head_weight, p.head_bias, p.head_channels = ptr(head_weight), ptr(head_bias), hc
+        if chunk is not None:
+            p.chunk, p.chunk_dtype = chunk.ctypes.data, self._dtype_code(chunk.dtype)
+            p.chunk_size[:] = list(chunk.shape)
+        p.in_origins, p.out_origins, p.mask, p.scale = ptr(in_origins), ptr(out_origins), ptr(mask), float(scale)
+        p.crop[:] = [int(v) for v in crop]
+        pooled = None
+        if op in ("head_blend", "conv3_head_blend"):
+            p.out_patch[:] = [int(v) for v in out_patch]
+            assert out.dtype == np.float32 and out.flags.c_contiguous and out.shape[0] == hc
+            p.out_size[:] = list(out.shape[1:])
+        else:
+            oc = hc if op == "head_sigmoid" else cout
+            shape = (z, 2 * y, 2 * x) if op == "convT" else (z, y // 2, x // 2) if op == "maxpool" else (z, y, x)
+            out = np.empty((nb, oc) + shape, np.float32)
+            if op == "conv3_pool":
+                pooled = np.empty((nb, cout, z, y // 2, x // 2), np.float32)
+                p.pooled = pooled.ctypes.data
+        p.out = out.ctypes.data
+        check(self._lib.cfb_debug_layer_host(self._h, C.byref(p)))
+        return (out, pooled) if pooled is not None else out

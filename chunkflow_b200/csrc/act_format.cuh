@@ -16,7 +16,8 @@
 // with powers of two chosen such that every term carries the scale alpha * beta:  gamma * mu = alpha and
 // lambda * delta = beta.  e4m3 spans 2^-9 .. 448, fp16 6e-8 .. 65504:
 //     alpha = 32, gamma = 1, lambda = 64, mu = 32         (activations: full accuracy up to |a| = 448, graceful --
-//                                                           fp16-level corrections -- up to 2047, clamped beyond)
+//                                                           fp16-level corrections -- up to 2047, clamped to
+//                                                           +-2047 beyond; NaN stays NaN in every record)
 //     beta  = 2^14 / wmax', delta = beta / 64              (per layer, wmax' = max |w| rounded up to a power of two)
 // The epilogue multiplies the accumulator by 1 / (alpha * beta).  Error of one product: the dropped a_lo w_lo (2^-24) plus
 // the e4m3 rounding (2^-4 relative) of two terms that are 2^-12 of the product: ~2^-16 worst case, ~2^-17.5 rms; the
@@ -33,6 +34,8 @@
 #include <cuda_fp8.h>
 
 #include <cstdint>
+
+#include "common.cuh"
 
 namespace cfb {
 
@@ -70,7 +73,8 @@ __device__ __forceinline__ void af_encode16(const float (&v)[16], uint4& h0, uin
   float l[16];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
-    const float s0 = fminf(fmaxf(v[2 * i] * kActAlpha, -kHalfMax), kHalfMax), s1 = fminf(fmaxf(v[2 * i + 1] * kActAlpha, -kHalfMax), kHalfMax);
+    const float s0 = min_nan(max_nan(v[2 * i] * kActAlpha, -kHalfMax), kHalfMax);
+    const float s1 = min_nan(max_nan(v[2 * i + 1] * kActAlpha, -kHalfMax), kHalfMax);
     const __half2 h = __floats2half2_rn(s0, s1);
     const float2 f = __half22float2(h);
     hw[i] = *reinterpret_cast<const uint32_t*>(&h);

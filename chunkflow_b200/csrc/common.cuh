@@ -17,6 +17,21 @@ struct Int3 {
 
 inline int64_t vol(const Int3& s) { return (int64_t)s.z * s.y * s.x; }
 
+#ifdef __CUDACC__
+// max / min that are NaN when either operand is NaN, as torch's max pooling and clamp are (fmaxf / fminf return the other
+// operand and would hide a broken weight from the output range check); one instruction each, like fmaxf / fminf
+__device__ __forceinline__ float max_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+__device__ __forceinline__ float min_nan(float a, float b) {
+  float r;
+  asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+#endif
+
 void set_last_error(const std::string& msg);
 
 struct CudaError : std::runtime_error {

@@ -815,12 +815,12 @@ int cfb_debug_net_forward_host(cfb_handle h, const float* h_patch, float* h_out)
   });
 }
 
-int cfb_debug_conv3_host(cfb_handle h, const float* h_in, int32_t cin, int32_t z, int32_t y, int32_t x,
-                         const float* h_weight, const float* h_bias, int32_t cout, int32_t relu, float* h_out) {
+int cfb_debug_layer_host(cfb_handle h, const cfb_layer_args* args) {
   return guarded([&]() -> int {
-    if (!h || !h_in || !h_weight || !h_bias || !h_out) throw std::invalid_argument("null argument");
+    if (!h || !args) throw std::invalid_argument("null argument");
+    if (args->struct_size != (int32_t)sizeof(cfb_layer_args)) throw std::invalid_argument("cfb_layer_args size mismatch");
     CFB_CUDA(cudaSetDevice(h->p.device));
-    return h->net.debug_conv3(h_in, cin, Int3{z, y, x}, h_weight, h_bias, cout, relu != 0, h_out, h->own_stream);
+    return h->net.debug_layer(*args, h->own_stream);
   });
 }
 

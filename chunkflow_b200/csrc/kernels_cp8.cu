@@ -56,7 +56,7 @@ __device__ __forceinline__ void store8(uint4* __restrict__ base, size_t plane0, 
     float s[8], l[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      s[i] = fminf(fmaxf(v[i] * kActAlpha, -kHalfMax), kHalfMax);
+      s[i] = min_nan(max_nan(v[i] * kActAlpha, -kHalfMax), kHalfMax);  // NaN stays NaN in H and L8 (af_encode16)
       const float h = __half2float(__float2half_rn(s[i]));
       l[i] = (s[i] - h) * kActLambda;
       s[i] = h;
@@ -178,7 +178,7 @@ maxpool_cp8_kernel(const uint4* __restrict__ in, uint4* __restrict__ out, int pa
       float v[8];
       load8(in, bc * fmt_planes(parts), parts, ipvol, iv, v);
 #pragma unroll
-      for (int e = 0; e < 8; ++e) m[e] = fmaxf(m[e], v[e]);
+      for (int e = 0; e < 8; ++e) m[e] = max_nan(m[e], v[e]);
     }
     store8(out, bc * fmt_planes(parts), parts, opvol, ov, m);
   }

@@ -105,7 +105,7 @@ maxpool_f32_kernel(const float* __restrict__ in, float* __restrict__ out, int64_
     const float* s = in + (p * Y + 2 * y) * X + 2 * x;
     const float2 a = *reinterpret_cast<const float2*>(s);
     const float2 c = *reinterpret_cast<const float2*>(s + X);
-    out[i] = fmaxf(fmaxf(a.x, a.y), fmaxf(c.x, c.y));
+    out[i] = max_nan(max_nan(a.x, a.y), max_nan(c.x, c.y));
   }
 }
 

@@ -475,7 +475,7 @@ conv3_wgmma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_consta
               for (int k = 0; k < 4; ++k) {
                 load16((2 * pr + (k >> 1)) * p.pitch + 2 * pc + (k & 1), cb, v);
 #pragma unroll
-                for (int i = 0; i < 16; ++i) m[i] = fmaxf(m[i], v[i]);
+                for (int i = 0; i < 16; ++i) m[i] = max_nan(m[i], v[i]);
               }
               const size_t pvox = ((size_t)z * (p.Y / 2) + (y0 / 2 + pr)) * (p.X / 2) + (x0 / 2 + pc);
               store16(m, cb, pvox, plane_vox / 4, pool16);

@@ -291,34 +291,215 @@ void Network::copy_raw_output_to_host(float* h_out, cudaStream_t s) {
   CFB_CUDA(cudaMemcpyAsync(h_out, f32(kOut), (size_t)cnet_ * vol(patch_) * sizeof(float), cudaMemcpyDeviceToHost, s));
 }
 
-int Network::debug_conv3(const float* h_in, int cin, Int3 size, const float* h_w, const float* h_b, int cout, bool relu,
-                         float* h_out, cudaStream_t s) {
-  const int64_t v = vol(size);
-  DeviceBuffer in((size_t)cin * v * 4), w((size_t)cout * cin * 27 * 4), b((size_t)cout * 4), out((size_t)cout * v * 4);
-  float *d_in = in.as<float>(), *d_out = out.as<float>();
-  CFB_CUDA(cudaMemcpyAsync(d_in, h_in, (size_t)cin * v * 4, cudaMemcpyHostToDevice, s));
-  CFB_CUDA(cudaMemcpyAsync(w.as(), h_w, (size_t)cout * cin * 27 * 4, cudaMemcpyHostToDevice, s));
-  CFB_CUDA(cudaMemcpyAsync(b.as(), h_b, (size_t)cout * 4, cudaMemcpyHostToDevice, s));
-  if (tensor_cores()) {
-    if (cin % 16) throw std::runtime_error("the wgmma convolution needs cin % 16 == 0");
-    const int P = parts();
-    DeviceBuffer cp8_in((size_t)cin * P * v * 2), cp8_out((size_t)cout * P * v * 2);
-    __half *c_in = cp8_in.as<__half>(), *c_out = cp8_out.as<__half>();
-    PackedConv pk;
-    pack_conv3_weights(h_w, h_b, cin, cout, fmt(), pk);
-    launch_planar_to_cp8(d_in, c_in, cin, fmt(), 1, size, s);
-    // exercise the two-source (concat) path whenever the channel count allows it
-    const int ca = cin >= 32 ? cin / 2 : cin, cb = cin - ca;
-    launch_conv3_wgmma(c_in, ca, cb ? c_in + (size_t)ca * P * v : nullptr, cb, pk, c_out, 1, size, relu, s);
-    launch_cp8_to_planar(c_out, d_out, cout, fmt(), 1, size, s);
-    CFB_CUDA(cudaMemcpyAsync(h_out, d_out, (size_t)cout * v * 4, cudaMemcpyDeviceToHost, s));
-    cudaError_t err = cudaStreamSynchronize(s);
-    free_packed(pk);
-    CFB_CUDA(err);
-    return CFB_OK;
+int Network::debug_layer(const cfb_layer_args& a, cudaStream_t s) {
+  const int nb = a.nb, ca = a.ca, cb = a.cb, cin = a.ca + a.cb, cout = a.cout, hc = a.head_channels;
+  const Int3 sz{a.size[0], a.size[1], a.size[2]}, half_sz{sz.z, sz.y / 2, sz.x / 2}, double_sz{sz.z, 2 * sz.y, 2 * sz.x};
+  const Int3 op{a.out_patch[0], a.out_patch[1], a.out_patch[2]}, crop{a.crop[0], a.crop[1], a.crop[2]};
+  const Int3 os{a.out_size[0], a.out_size[1], a.out_size[2]}, cs{a.chunk_size[0], a.chunk_size[1], a.chunk_size[2]};
+  if (nb < 1 || sz.z < 1 || sz.y < 1 || sz.x < 1 || ca < 0 || cb < 0) throw std::invalid_argument("debug_layer: bad shape");
+  const bool tc = tensor_cores(), first_from_chunk = a.op == CFB_LAYER_FIRST && a.chunk;
+  const bool blend = a.op == CFB_LAYER_HEAD_BLEND || a.op == CFB_LAYER_CONV3_HEAD_BLEND;
+  const bool head = blend || a.op == CFB_LAYER_HEAD_SIGMOID;
+  if ((a.op == CFB_LAYER_CONV3_POOL || a.op == CFB_LAYER_MAXPOOL) && ((sz.y & 1) || (sz.x & 1)))
+    throw std::invalid_argument("debug_layer: pooling needs even y and x");
+  if (a.op == CFB_LAYER_FIRST && (ca != 1 || cb)) throw std::invalid_argument("debug_layer: the first layer reads one channel");
+  if (head && (hc < 1 || hc > 8)) throw std::invalid_argument("debug_layer: 1 to 8 head channels");
+  if (blend && (!a.mask || !a.out_origins || vol(op) < 1 || vol(os) < 1 || op.z + crop.z > sz.z || op.y + crop.y > sz.y ||
+                op.x + crop.x > sz.x || crop.z < 0 || crop.y < 0 || crop.x < 0))
+    throw std::invalid_argument("debug_layer: bad blend geometry");
+  const CrossChecks checks = read_cross_checks();
+  const int F = fmt(), P = parts();
+
+  std::vector<DeviceBuffer> bufs;  // every allocation of this call
+  auto alloc = [&](size_t bytes) { bufs.emplace_back(bytes); return bufs.back().as(); };
+  auto upload = [&](const void* h, size_t bytes) {
+    if (!h) throw std::invalid_argument("debug_layer: missing input array");
+    void* d = alloc(bytes);
+    CFB_CUDA(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, s));
+    return static_cast<float*>(d);
+  };
+  auto download = [&](float* h, const float* d, size_t bytes) {
+    if (!h) throw std::invalid_argument("debug_layer: missing output array");
+    CFB_CUDA(cudaMemcpyAsync(h, d, bytes, cudaMemcpyDeviceToHost, s));
+  };
+  // planar fp32 (nb, c, e) <-> CP8 of the mode's format; 128 channels half-major (kernels_conv.cuh): one conversion per
+  // (half, patch)
+  auto to_cp8 = [&](const float* d, int c, Int3 e) {
+    if (c % 8 || (c > 64 && c != 128)) throw std::invalid_argument("debug_layer: CP8 tensors have 8 .. 64 or 128 channels");
+    __half* t = static_cast<__half*>(alloc((size_t)nb * c * P * vol(e) * sizeof(__half)));
+    if (c <= 64) launch_planar_to_cp8(d, t, c, F, nb, e, s);
+    else
+      for (int h = 0; h < 2; ++h)
+        for (int b = 0; b < nb; ++b)
+          launch_planar_to_cp8(d + ((size_t)b * c + h * 64) * vol(e), t + ((size_t)h * nb + b) * 64 * P * vol(e), 64, F, 1, e, s);
+    return t;
+  };
+  auto from_cp8 = [&](const __half* t, int c, Int3 e) {
+    float* d = static_cast<float*>(alloc((size_t)nb * c * vol(e) * sizeof(float)));
+    if (c <= 64) launch_cp8_to_planar(t, d, c, F, nb, e, s);
+    else
+      for (int h = 0; h < 2; ++h)
+        for (int b = 0; b < nb; ++b)
+          launch_cp8_to_planar(t + ((size_t)h * nb + b) * 64 * P * vol(e), d + ((size_t)b * c + h * 64) * vol(e), 64, F, 1, e, s);
+    return d;
+  };
+  auto cp8_out = [&](int c, Int3 e) { return static_cast<__half*>(alloc((size_t)nb * c * P * vol(e) * sizeof(__half))); };
+  auto f32_out = [&](int c, Int3 e) { return static_cast<float*>(alloc((size_t)nb * c * vol(e) * sizeof(float))); };
+  struct Packed {
+    PackedConv p;
+    ~Packed() { free_packed(p); }
+  } pk;
+
+  const float* d_a = first_from_chunk ? nullptr : upload(a.a, (size_t)nb * ca * vol(sz) * sizeof(float));
+  const float* d_b = cb ? upload(a.b, (size_t)nb * cb * vol(sz) * sizeof(float)) : nullptr;
+  const __half* c_a = tc && a.op != CFB_LAYER_FIRST ? to_cp8(d_a, ca, sz) : nullptr;
+  const __half* c_b = tc && cb ? to_cp8(d_b, cb, sz) : nullptr;
+  const float* d_hw = head ? upload(a.head_weight, (size_t)hc * 16 * sizeof(float)) : nullptr;
+  const float* d_hb = head ? upload(a.head_bias, (size_t)hc * sizeof(float)) : nullptr;
+  PatchPos* d_pp = nullptr;
+  if (blend || first_from_chunk) {
+    std::vector<PatchPos> pp(nb);
+    for (int b = 0; b < nb; ++b) {
+      if (first_from_chunk) {
+        pp[b].iz = a.in_origins[3 * b]; pp[b].iy = a.in_origins[3 * b + 1]; pp[b].ix = a.in_origins[3 * b + 2];
+        if (pp[b].iz < 0 || pp[b].iy < 0 || pp[b].ix < 0 || pp[b].iz + sz.z > cs.z || pp[b].iy + sz.y > cs.y || pp[b].ix + sz.x > cs.x)
+          throw std::invalid_argument("debug_layer: patch outside the chunk");
+      }
+      if (blend) { pp[b].oz = a.out_origins[3 * b]; pp[b].oy = a.out_origins[3 * b + 1]; pp[b].ox = a.out_origins[3 * b + 2]; }
+    }
+    d_pp = reinterpret_cast<PatchPos*>(upload(pp.data(), nb * sizeof(PatchPos)));
   }
-  launch_conv3_f32(d_in, cin, nullptr, 0, w.as<float>(), b.as<float>(), d_out, cout, 1, size, relu, s);
-  CFB_CUDA(cudaMemcpyAsync(h_out, d_out, (size_t)cout * v * 4, cudaMemcpyDeviceToHost, s));
+  float* d_out = nullptr;   // blend: the accumulated output chunk
+  const float* d_mask = nullptr;
+  if (blend) {
+    d_mask = upload(a.mask, vol(op) * sizeof(float));
+    d_out = upload(a.out, (size_t)hc * vol(os) * sizeof(float));
+  }
+  auto blend_tail = [&]() { return ConvTail{d_hw, d_hb, d_pp, d_mask, d_out, hc, op, crop, os, a.scale}; };
+
+  switch (a.op) {
+    case CFB_LAYER_CONV3: case CFB_LAYER_CONV3_POOL: case CFB_LAYER_CONV3_HEAD_BLEND: {
+      const bool pool = a.op == CFB_LAYER_CONV3_POOL, tail = a.op == CFB_LAYER_CONV3_HEAD_BLEND;
+      if (tail && (cin != 16 || cout != 16)) throw std::invalid_argument("debug_layer: the fused tail follows a 16 -> 16 layer");
+      const bool relu = tail || a.relu;
+      if (!tc) {
+        const float *w = upload(a.weight, (size_t)cout * cin * 27 * sizeof(float)), *bias = upload(a.bias, cout * sizeof(float));
+        float* o = f32_out(cout, sz);
+        launch_conv3_f32(d_a, ca, d_b, cb, w, bias, o, cout, nb, sz, relu, s);
+        if (tail) {
+          float* net = f32_out(hc, sz);
+          launch_head_sigmoid_f32(o, d_hw, d_hb, net, 16, hc, nb, sz, s);
+          launch_blend_patches(net, hc, sz, op, crop, d_mask, d_pp, nb, d_out, hc, os, a.scale, s);
+          break;
+        }
+        download(a.out, o, (size_t)nb * cout * vol(sz) * sizeof(float));
+        if (pool) {
+          float* po = f32_out(cout, half_sz);
+          launch_maxpool_f32(o, po, cout, nb, sz, s);
+          download(a.pooled, po, (size_t)nb * cout * vol(half_sz) * sizeof(float));
+        }
+        break;
+      }
+      if (!a.weight || !a.bias) throw std::invalid_argument("debug_layer: missing weights");
+      pack_conv3_weights(a.weight, a.bias, cin, cout, F, pk.p);
+      __half* o = cp8_out(cout, sz);
+      __half* po = pool ? cp8_out(cout, half_sz) : nullptr;
+      const ConvTail t = blend_tail();
+      const bool fuse_tail = tail && !checks.no_fused_tail, fuse_pool = pool && !checks.no_pool_fusion;
+      launch_conv3_wgmma(c_a, ca, c_b, cb, pk.p, o, nb, sz, relu, s, fuse_tail ? &t : nullptr, fuse_pool ? po : nullptr);
+      if (tail) {
+        if (!fuse_tail) launch_head_blend_cp8(o, d_hw, d_hb, 16, hc, F, sz, op, crop, d_mask, d_pp, nb, d_out, hc, os, a.scale, s);
+        break;
+      }
+      download(a.out, from_cp8(o, cout, sz), (size_t)nb * cout * vol(sz) * sizeof(float));
+      if (pool) {
+        if (!fuse_pool) launch_maxpool_cp8(o, po, cout, F, nb, sz, s);
+        download(a.pooled, from_cp8(po, cout, half_sz), (size_t)nb * cout * vol(half_sz) * sizeof(float));
+      }
+      break;
+    }
+    case CFB_LAYER_CONVT: {
+      const float *w = upload(a.weight, (size_t)ca * cout * 4 * sizeof(float)), *bias = upload(a.bias, cout * sizeof(float));
+      if (!tc) {
+        float* o = f32_out(cout, double_sz);
+        launch_convT_f32(d_a, w, bias, o, ca, cout, nb, sz, s);
+        download(a.out, o, (size_t)nb * cout * vol(double_sz) * sizeof(float));
+        break;
+      }
+      __half* o = cp8_out(cout, double_sz);
+      if (checks.simt_convt) {
+        launch_convT_cp8(c_a, w, bias, o, ca, cout, F, nb, sz, s);
+      } else {
+        pack_convT_weights(a.weight, a.bias, ca, cout, F, pk.p);
+        launch_convT_wgmma(c_a, pk.p, o, nb, sz, s);
+      }
+      download(a.out, from_cp8(o, cout, double_sz), (size_t)nb * cout * vol(double_sz) * sizeof(float));
+      break;
+    }
+    case CFB_LAYER_MAXPOOL: {
+      if (!tc) {
+        float* o = f32_out(ca, half_sz);
+        launch_maxpool_f32(d_a, o, ca, nb, sz, s);
+        download(a.out, o, (size_t)nb * ca * vol(half_sz) * sizeof(float));
+        break;
+      }
+      __half* o = cp8_out(ca, half_sz);
+      launch_maxpool_cp8(c_a, o, ca, F, nb, sz, s);
+      download(a.out, from_cp8(o, ca, half_sz), (size_t)nb * ca * vol(half_sz) * sizeof(float));
+      break;
+    }
+    case CFB_LAYER_FIRST: {
+      if (!a.weight || !a.bias) throw std::invalid_argument("debug_layer: missing weights");
+      const void* chunk = nullptr;
+      if (first_from_chunk) {
+        if (a.chunk_dtype != CFB_DTYPE_U8 && a.chunk_dtype != CFB_DTYPE_F32) throw std::invalid_argument("debug_layer: uint8 or float32 chunk");
+        chunk = upload(a.chunk, vol(cs) * (a.chunk_dtype == CFB_DTYPE_U8 ? 1 : sizeof(float)));
+      }
+      if (!tc) {
+        const float *w = upload(a.weight, 16 * 27 * sizeof(float)), *bias = upload(a.bias, 16 * sizeof(float));
+        const float* in = d_a;
+        if (chunk) {
+          if (sz.x % 4) throw std::invalid_argument("debug_layer: the patch extraction needs x % 4 == 0");
+          float* ex = f32_out(1, sz);
+          launch_extract_patches(chunk, a.chunk_dtype, cs, d_pp, nb, sz, ex, s);
+          in = ex;
+        }
+        float* o = f32_out(16, sz);
+        launch_conv3_f32(in, 1, nullptr, 0, w, bias, o, 16, nb, sz, /*relu=*/true, s);
+        download(a.out, o, (size_t)nb * 16 * vol(sz) * sizeof(float));
+        break;
+      }
+      FirstConvW W{};
+      for (int t = 0; t < 27; ++t)
+        for (int c = 0; c < 16; ++c) W.w[t][c] = a.weight[c * 27 + t];
+      for (int c = 0; c < 16; ++c) W.b[c] = a.bias[c];
+      __half* o = cp8_out(16, sz);
+      if (chunk) launch_first_conv_cp8(chunk, a.chunk_dtype, cs, d_pp, nb, sz, W, o, F, s);
+      else launch_first_conv_cp8_from_patches(d_a, nb, sz, W, o, F, s);
+      download(a.out, from_cp8(o, 16, sz), (size_t)nb * 16 * vol(sz) * sizeof(float));
+      break;
+    }
+    case CFB_LAYER_HEAD_SIGMOID: case CFB_LAYER_HEAD_BLEND: {
+      if (ca != 16 || cb) throw std::invalid_argument("debug_layer: the head reads 16 channels");
+      float* net = f32_out(hc, sz);
+      if (a.op == CFB_LAYER_HEAD_BLEND && tc) {
+        launch_head_blend_cp8(c_a, d_hw, d_hb, 16, hc, F, sz, op, crop, d_mask, d_pp, nb, d_out, hc, os, a.scale, s);
+        break;
+      }
+      if (tc) launch_head_sigmoid_cp8(c_a, d_hw, d_hb, net, 16, hc, F, nb, sz, s);
+      else launch_head_sigmoid_f32(d_a, d_hw, d_hb, net, 16, hc, nb, sz, s);
+      if (a.op == CFB_LAYER_HEAD_BLEND) launch_blend_patches(net, hc, sz, op, crop, d_mask, d_pp, nb, d_out, hc, os, a.scale, s);
+      else download(a.out, net, (size_t)nb * hc * vol(sz) * sizeof(float));
+      break;
+    }
+    case CFB_LAYER_ROUND_TRIP:
+      if (!tc) throw std::invalid_argument("debug_layer: the simt mode keeps fp32 activations");
+      download(a.out, from_cp8(c_a, ca, sz), (size_t)nb * ca * vol(sz) * sizeof(float));
+      break;
+    default:
+      throw std::invalid_argument("debug_layer: unknown op");
+  }
+  if (blend) download(a.out, d_out, (size_t)hc * vol(os) * sizeof(float));
   CFB_CUDA(cudaStreamSynchronize(s));
   return CFB_OK;
 }

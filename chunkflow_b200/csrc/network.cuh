@@ -44,8 +44,8 @@ class Network {
   void set_profiling(bool on);
   void layer_timing(std::vector<std::string>& names, std::vector<float>& ms, std::vector<int64_t>& launches);
 
-  int debug_conv3(const float* h_in, int cin, Int3 size, const float* h_w, const float* h_b, int cout, bool relu,
-                  float* h_out, cudaStream_t s);
+  // One step of the layer table on host arrays (cfb_debug_layer_host); the network's own weights and workspace are not used.
+  int debug_layer(const cfb_layer_args& a, cudaStream_t s);
 
  private:
   // How the network ends: head + blend in the epilogue of the last convolution, head + blend (tensor cores: one CUDA-core

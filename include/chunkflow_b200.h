@@ -214,11 +214,56 @@ int cfb_layer_timing(cfb_handle h, int32_t capacity, int32_t* count, char (*name
 
 /* Test hook: raw network output (before crop/mask) of one host patch, (Cnet,pz,py,px). */
 int cfb_debug_net_forward_host(cfb_handle h, const float* h_patch, float* h_out);
-/* Test hook: one 3x3x3 convolution layer run through the engine's precision path.
- * in (cin,z,y,x) fp32 host, weight (cout,cin,3,3,3), bias (cout) -> out (cout,z,y,x). */
-int cfb_debug_conv3_host(cfb_handle h, const float* h_in, int32_t cin, int32_t z, int32_t y, int32_t x,
-                         const float* h_weight, const float* h_bias, int32_t cout, int32_t relu,
-                         float* h_out);
+/* Test hook: one step of the U-Net layer table run through the kernels of the engine's precision mode, on fp32 planar
+ * host arrays.  The tensor-core modes convert the sources to the mode's activation format (a 128-channel tensor half-major)
+ * and the results back; the cross-check switches CFB_NO_POOL_FUSION, CFB_SIMT_CONVT and CFB_NO_FUSED_TAIL are honoured as
+ * in inference.  Shapes (nb patches, c = ca + cb channels, size = z, y, x of the step's input):
+ *   CONV3            a (nb,ca,size) and b (nb,cb,size), two separate allocations concatenated as torch.cat([a, b]);
+ *                    weight (cout,c,3,3,3), bias (cout) -> out (nb,cout,size); relu optional
+ *   CONV3_POOL       the same, and pooled (nb,cout,z,y/2,x/2) = its (1,2,2) max pool
+ *   CONVT            a (nb,ca,size), weight (ca,cout,1,2,2), bias (cout) -> out (nb,cout,z,2y,2x)
+ *   MAXPOOL          a (nb,ca,size) -> out (nb,ca,z,y/2,x/2)
+ *   FIRST            weight (16,1,3,3,3), bias (16) -> out (nb,16,size), ReLU; from a (nb,1,size), or, if chunk is
+ *                    not NULL, from the uint8 (normalised by 1/255) or float32 chunk at in_origins
+ *   HEAD_SIGMOID     a (nb,16,size), head_weight (head_channels,16), head_bias -> out (nb,head_channels,size)
+ *   HEAD_BLEND       the same head, then crop, x mask (out_patch) x scale, accumulated into out (head_channels,out_size)
+ *                    at out_origins (a patch may stick out of out_size: clipped)
+ *   CONV3_HEAD_BLEND the 16 -> 16 CONV3 (ReLU) and HEAD_BLEND in one step: the fused epilogue on the tensor cores
+ *   ROUND_TRIP       a (nb,ca,size) -> the mode's activation format -> out (nb,ca,size) */
+#define CFB_LAYER_CONV3 0
+#define CFB_LAYER_CONV3_POOL 1
+#define CFB_LAYER_CONVT 2
+#define CFB_LAYER_MAXPOOL 3
+#define CFB_LAYER_FIRST 4
+#define CFB_LAYER_HEAD_SIGMOID 5
+#define CFB_LAYER_HEAD_BLEND 6
+#define CFB_LAYER_CONV3_HEAD_BLEND 7
+#define CFB_LAYER_ROUND_TRIP 8
+typedef struct cfb_layer_args {
+  int32_t struct_size; /* = sizeof(cfb_layer_args) */
+  int32_t op;          /* CFB_LAYER_* */
+  int32_t nb;
+  int32_t size[3];
+  int32_t ca, cb, cout, relu;
+  const float* a;
+  const float* b;
+  const float* weight;
+  const float* bias;
+  const float* head_weight;
+  const float* head_bias;
+  int32_t head_channels;
+  int32_t chunk_dtype; /* CFB_DTYPE_U8 or CFB_DTYPE_F32 */
+  const void* chunk;
+  int32_t chunk_size[3];
+  int32_t out_patch[3], crop[3], out_size[3];
+  const int32_t* in_origins;  /* (nb, 3) */
+  const int32_t* out_origins; /* (nb, 3) */
+  const float* mask;
+  float scale;
+  float* out;
+  float* pooled;
+} cfb_layer_args;
+int cfb_debug_layer_host(cfb_handle h, const cfb_layer_args* args);
 
 /* ---------------------------------------------------------------------------------------------
  * Operators either side of `inference`, on device memory (SURVEY.md section 8 f3): the chunk can stay in HBM

@@ -128,23 +128,17 @@ def test_unet3l_readme_config_against_oracle(unet_model):
     assert inf.timing["launches"] > 0
 
 
-def _conv3_case(prec, cin, cout, size, atol, round_operands=False):
-    import torch
-    rng = np.random.default_rng(cin * 100 + cout)
-    x = rng.standard_normal((cin,) + size).astype(np.float32)
-    w = (rng.standard_normal((cout, cin, 3, 3, 3)) / np.sqrt(27 * cin)).astype(np.float32)
-    b = rng.standard_normal(cout).astype(np.float32)
-    eng = _native.Engine(input_patch_size=(8, 32, 32), output_patch_size=(8, 32, 32), output_patch_overlap=(2, 8, 8),
-                         output_crop_margin=(0, 0, 0), framework=_native.FRAMEWORK_IDENTITY, precision=prec)
-    got = eng.debug_conv3(x, w, b, relu=True)
-    xt, wt = torch.from_numpy(x), torch.from_numpy(w)
-    ref = torch.relu(torch.nn.functional.conv3d(xt[None], wt, torch.from_numpy(b), padding=1))[0].numpy()
-    np.testing.assert_allclose(got, ref, rtol=0, atol=atol)
+def _conv3_case(mode, cin, cout, size):
+    """One layer through cfb_debug_layer_host against the float64 reference and the relative bound of test_gpu_layers.py;
+    for cin >= 32 the input is fed as two sources (the decoders' concat)."""
+    from test_gpu_layers import conv_case
+    cb = cin // 2 if cin >= 32 else 0
+    conv_case(mode, cin - cb, cb, cout, size)
 
 
 @pytest.mark.parametrize("cin,cout,size", [(1, 16, (5, 20, 36)), (16, 16, (4, 16, 70)), (48, 32, (3, 9, 13)), (64, 64, (6, 8, 8))])
 def test_conv3_layer_simt_against_torch(cin, cout, size):
-    _conv3_case(_native.PRECISION_F32_SIMT, cin, cout, size, 2e-5)
+    _conv3_case("simt", cin, cout, size)
 
 
 # (cin, cout, size): dense M tiles with junk columns, row-aligned 128-voxel tiles with two x tiles,
@@ -156,8 +150,7 @@ UMMA_CASES = [(16, 16, (3, 8, 40)), (16, 16, (4, 16, 70)), (32, 32, (3, 12, 20))
 
 @pytest.mark.parametrize("cin,cout,size", UMMA_CASES)
 def test_conv3_layer_tcgen05_split_against_torch(cin, cout, size):
-    # hi/lo split operands: ~22 significant bits, fp32 accumulation
-    _conv3_case(_native.PRECISION_F16X3_UMMA, cin, cout, size, 5e-5)
+    _conv3_case("f16x3", cin, cout, size)
 
 
 @pytest.mark.parametrize("zstack", ["2", "3", "4", "8"])
@@ -166,9 +159,9 @@ def test_conv3_layer_tcgen05_split_against_torch(cin, cout, size):
 def test_conv3_layer_tcgen05_zstacked_kernel(monkeypatch, zstack, cin, cout, size):
     """The convolution split along z into blocks of T output planes per CTA (each block loads its own halo planes), forced."""
     monkeypatch.setenv("CFB_FORCE_ZBLOCK", zstack)
-    _conv3_case(_native.PRECISION_F16X3_UMMA, cin, cout, size, 5e-5)
+    _conv3_case("f16x3", cin, cout, size)
     if cin == 16:
-        _conv3_case(_native.PRECISION_F16_UMMA, cin, cout, size, 1e-2)
+        _conv3_case("f16", cin, cout, size)
 
 
 @pytest.mark.parametrize("zstack", ["2", "3", "4"])
@@ -179,29 +172,26 @@ def test_conv3_layer_tcgen05_tmem_shift_kernel(monkeypatch, zstack, cin, cout, s
     instead of resident, forced."""
     monkeypatch.setenv("CFB_FORCE_ZBLOCK", zstack)
     monkeypatch.setenv("CFB_FORCE_WEIGHT_RING", "1")
-    _conv3_case(_native.PRECISION_F16X3_UMMA, cin, cout, size, 5e-5)
+    _conv3_case("f16x3", cin, cout, size)
     if cin == 16:
-        _conv3_case(_native.PRECISION_F16_UMMA, cin, cout, size, 1e-2)
+        _conv3_case("f16", cin, cout, size)
 
 
 @pytest.mark.parametrize("cin,cout,size", UMMA_CASES)
 def test_conv3_layer_tcgen05_f16f8_against_torch(cin, cout, size):
-    # fp16 main product + one e4m3 (K = 32) product for both correction terms: ~2^-16 relative per product
-    # (inputs ~N(0,1), outputs of magnitude ~5: fp16 alone is asserted at 1e-2 below, the hi/lo split at 5e-5)
-    _conv3_case(_native.PRECISION_F16F8_UMMA, cin, cout, size, 4e-4)
+    _conv3_case("f16f8", cin, cout, size)
 
 
 @pytest.mark.parametrize("zstack", ["2", "3", "4"])
 @pytest.mark.parametrize("cin,cout,size", [(16, 16, (9, 16, 70)), (32, 32, (5, 12, 20)), (64, 32, (4, 16, 16)), (16, 16, (1, 7, 9))])
 def test_conv3_layer_f16f8_forced_zstack(monkeypatch, zstack, cin, cout, size):
     monkeypatch.setenv("CFB_FORCE_ZBLOCK", zstack)
-    _conv3_case(_native.PRECISION_F16F8_UMMA, cin, cout, size, 4e-4)
+    _conv3_case("f16f8", cin, cout, size)
 
 
 @pytest.mark.parametrize("cin,cout,size", UMMA_CASES[:4])
 def test_conv3_layer_tcgen05_fp16_against_torch(cin, cout, size):
-    # single-pass fp16: 11-bit operands and 11-bit stored outputs on values of magnitude ~5
-    _conv3_case(_native.PRECISION_F16_UMMA, cin, cout, size, 1e-2)
+    _conv3_case("f16", cin, cout, size)
 
 
 def test_plugin_level_patch_inferencer(unet_model):

@@ -63,25 +63,15 @@ def test_depth4_readme_geometry_against_oracle(checkpoint):
     assert err <= NET_ATOL_F32
 
 
-@pytest.mark.parametrize("precision,atol", [(_native.PRECISION_F32_SIMT, 2e-5), (_native.PRECISION_F16X3_UMMA, 5e-5),
-                                            (_native.PRECISION_F16F8_UMMA, 4e-4), (_native.PRECISION_F16_UMMA, 1e-2)])
+@pytest.mark.parametrize("mode", ["simt", "f16x3", "f16f8", "f16"])
 @pytest.mark.parametrize("cin,cout,size", [(64, 128, (3, 9, 13)), (128, 128, (4, 16, 16)), (128, 64, (3, 8, 20)),
                                            (64, 64, (5, 6, 10))])
-def test_wide_layer_against_torch(precision, atol, cin, cout, size):
-    """One layer through cfb_debug_conv3_host; for cin >= 32 the input is fed as two concatenated halves, so 128 -> 64 is
-    also the decoder's 64 + 64 concat."""
-    import torch
-    rng = np.random.default_rng(cin * 1000 + cout)
-    x = rng.standard_normal((cin,) + size).astype(np.float32)
-    w = (rng.standard_normal((cout, cin, 3, 3, 3)) / np.sqrt(27 * cin)).astype(np.float32)
-    b = rng.standard_normal(cout).astype(np.float32)
-    eng = _native.Engine(input_patch_size=(8, 32, 32), output_patch_size=(8, 32, 32), output_patch_overlap=(2, 8, 8),
-                         output_crop_margin=(0, 0, 0), framework=_native.FRAMEWORK_IDENTITY, precision=precision)
-    got = eng.debug_conv3(x, w, b, relu=True)
-    ref = torch.relu(torch.nn.functional.conv3d(torch.from_numpy(x)[None], torch.from_numpy(w), torch.from_numpy(b),
-                                                padding=1))[0].numpy()
-    np.testing.assert_allclose(got, ref, rtol=0, atol=atol)
-    eng.close()
+def test_wide_layer_against_torch(mode, cin, cout, size):
+    """One layer through cfb_debug_layer_host against the float64 reference and bound of test_gpu_layers.py, at three
+    patches when a tensor has 128 channels (stored half-major); for cin >= 32 the input is fed as two separately allocated
+    halves, so 128 -> 64 is also the decoder's 64 + 64 concat."""
+    from test_gpu_layers import conv_case
+    conv_case(mode, cin // 2, cin // 2, cout, size, nb=3 if 128 in (cin, cout) else 1)
 
 
 def _run(monkeypatch, checkpoint, env, img, precision=None, batch=3):
