@@ -41,6 +41,7 @@ EXPORTS = (
     "cfb_gaussian_filter_workspace", "cfb_gaussian_filter_device", "cfb_median_filter_device",
     "cfb_clahe_workspace", "cfb_clahe_device",
     "cfb_mesh_workspace", "cfb_mesh_count_device", "cfb_mesh_buffer_bytes", "cfb_mesh_device", "cfb_mesh_read", "cfb_mesh_simplify_host",
+    "cfb_skeleton_workspace", "cfb_edt_workspace", "cfb_edt_device", "cfb_skeleton_count_device", "cfb_skeleton_device", "cfb_skeleton_read",
 )
 
 
@@ -192,6 +193,7 @@ def load() -> C.CDLL:
     lib.cfb_clahe_workspace.argtypes = [i64, i64, i64, i32, i32, C.POINTER(i64)]
     lib.cfb_clahe_device.argtypes = [vp, vp, i64, i64, i64, C.c_double, i32, i32, vp, i64, vp]
     bind_mesh(lib)
+    bind_skeleton(lib)
     for name in EXPORTS:
         getattr(lib, name)   # every declared symbol must be there
     _lib = lib
@@ -709,6 +711,87 @@ def mesh_simplify_host(vertices, faces, simplification_factor: int, max_simplifi
 def _mesh_check(lib, code: int) -> None:
     if code != OK:
         raise NativeError(code, lib.cfb_last_error().decode("utf-8", "replace"))
+
+
+# ---- `skeletonize` (include/chunkflow_b200.h) ----
+SKELETON_STATS = ("sweeps", "rounds", "paths", "skeleton_voxels", "relax_ms", "sort_ms", "rounds_ms", "trace_ms")
+
+
+def bind_skeleton(lib: C.CDLL) -> None:
+    """Argument types of the skeleton entry points (also for the host emulation of csrc/skeleton.cu)."""
+    vp, i32, i64, pi64 = C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_int64)
+    lib.cfb_skeleton_workspace.argtypes = [i64, i64, i64, pi64]
+    lib.cfb_edt_workspace.argtypes = [i64, i64, i64, pi64]
+    lib.cfb_edt_device.argtypes = [vp, i32, i64, i64, i64, vp, vp, vp, vp]
+    lib.cfb_skeleton_count_device.argtypes = [vp, i32, i64, i64, i64, vp, vp, i64, i64, vp, pi64, pi64, pi64, vp]
+    lib.cfb_skeleton_device.argtypes = [vp, i32, i64, i64, i64, vp, vp, i32, vp, i64, i64, vp, i64, pi64, vp, vp]
+    lib.cfb_skeleton_read.argtypes = [vp, i64, i64, i64, vp, i64, i64, i64, pi64, vp, vp, vp, vp, vp, vp, vp]
+
+
+def _voxel_size(voxel_size) -> np.ndarray:
+    vs = np.ascontiguousarray(voxel_size, np.float64)
+    if vs.shape != (3,):
+        raise ValueError("the voxel size is (z, y, x)")
+    return vs
+
+
+def skeleton_workspace(zyx, lib=None) -> int:
+    """Bytes of the per-voxel workspace of a (z, y, x) volume (no device needed)."""
+    lib, out = lib or load(), C.c_int64()
+    _mesh_check(lib, lib.cfb_skeleton_workspace(*(int(v) for v in zyx), C.byref(out)))
+    return int(out.value)
+
+
+def edt_workspace(zyx, lib=None) -> int:
+    """Bytes of the workspace of the distance transform alone (no device needed)."""
+    lib, out = lib or load(), C.c_int64()
+    _mesh_check(lib, lib.cfb_edt_workspace(*(int(v) for v in zyx), C.byref(out)))
+    return int(out.value)
+
+
+def edt_device(d_labels: int, dtype: int, zyx, voxel_size, d_out: int, d_workspace: int, stream: int = 0, lib=None) -> None:
+    """``d_out`` (float32) = the multi-label distance to the boundary of the segmentation at ``d_labels``."""
+    vs, lib = _voxel_size(voxel_size), lib or load()
+    _mesh_check(lib, lib.cfb_edt_device(C.c_void_p(d_labels), int(dtype), *(int(v) for v in zyx), _ptr(vs), C.c_void_p(d_out),
+                                        C.c_void_p(d_workspace), C.c_void_p(stream)))
+
+
+def skeleton_count_device(d_labels: int, dtype: int, zyx, voxel_size, d_skip: int, num_skip: int, dust_threshold: int, d_workspace: int,
+                          stream: int = 0, lib=None):
+    """-> (objects, their voxels, buffer bytes) of the segmentation at ``d_labels`` (synchronises the stream)."""
+    vs, lib = _voxel_size(voxel_size), lib or load()
+    k, m, nb = C.c_int64(), C.c_int64(), C.c_int64()
+    _mesh_check(lib, lib.cfb_skeleton_count_device(C.c_void_p(d_labels), int(dtype), *(int(v) for v in zyx), _ptr(vs),
+                                                   C.c_void_p(d_skip or None), int(num_skip), int(dust_threshold), C.c_void_p(d_workspace),
+                                                   C.byref(k), C.byref(m), C.byref(nb), C.c_void_p(stream)))
+    return int(k.value), int(m.value), int(nb.value)
+
+
+def skeleton_device(d_labels: int, dtype: int, zyx, voxel_size, scale: float, const: float, pdrf_scale: float, pdrf_exponent: int,
+                    d_workspace: int, counts, d_buffer: int, stream: int = 0, lib=None):
+    """Every skeleton on the device into ``d_buffer`` -> (skeleton voxels, {stat: value}) (synchronises the stream)."""
+    vs, lib = _voxel_size(voxel_size), lib or load()
+    prm = np.array([scale, const, pdrf_scale], np.float64)
+    st = np.zeros(len(SKELETON_STATS), np.float64)
+    K, m, nb = (int(v) for v in counts)
+    S = C.c_int64()
+    _mesh_check(lib, lib.cfb_skeleton_device(C.c_void_p(d_labels), int(dtype), *(int(v) for v in zyx), _ptr(vs), _ptr(prm), int(pdrf_exponent),
+                                             C.c_void_p(d_workspace), K, m, C.c_void_p(d_buffer or None), nb, C.byref(S), _ptr(st),
+                                             C.c_void_p(stream)))
+    return int(S.value), dict(zip(SKELETON_STATS, st.tolist()))
+
+
+def skeleton_read(d_buffer: int, zyx, voxel_size, counts, num_skeleton_voxels: int, stream: int = 0, lib=None) -> dict:
+    """The skeletons of skeleton_device -> {id: (vertices float32 (N, 3) x y z, edges uint32 (M, 2), radii float32 (N,))}."""
+    vs, lib = _voxel_size(voxel_size), lib or load()
+    K, m, _ = (int(v) for v in counts)
+    S = int(num_skeleton_voxels)
+    ids, vo, eo = np.empty(max(K, 1), np.uint64), np.empty(K + 1, np.int64), np.empty(K + 1, np.int64)
+    verts, edges, radii = np.empty((S, 3), np.float32), np.empty((max(S - K, 0), 2), np.uint32), np.empty(S, np.float32)
+    nl = C.c_int64()
+    _mesh_check(lib, lib.cfb_skeleton_read(C.c_void_p(d_buffer or None), *(int(v) for v in zyx), _ptr(vs), K, m, S, C.byref(nl), _ptr(ids),
+                                           _ptr(vo), _ptr(eo), _ptr(verts), _ptr(edges), _ptr(radii), C.c_void_p(stream)))
+    return {int(ids[i]): (verts[vo[i]:vo[i + 1]], edges[eo[i]:eo[i + 1]], radii[vo[i]:vo[i + 1]]) for i in range(int(nl.value))}
 
 
 def device_memory(device: int = 0) -> tuple:

@@ -18,6 +18,7 @@ bookkeeping of the reference's ``Chunk`` and mirrors, name for name, the referen
     median_filter        reference plugins/median_filter.py:4-7         (plugin -> scipy.ndimage.median_filter)
     clahe                reference plugins/clahe.py                     (plugin -> cv2.createCLAHE(...).apply)
     mesh                 reference flow/mesh.py                         (MeshOperator -> zmesh; rules restated)
+    skeletonize          reference plugins/skeletonize.py               (plugin -> kimimaro; rules restated)
 
 so that ``create-chunk | normalize-contrast | inference | crop-margin | quantize`` moves the image to the GPU once and
 brings a uint8 thumbnail (or nothing) back instead of the 12-byte-per-voxel affinity map.  There is no CPU fallback.
@@ -700,6 +701,27 @@ class DeviceChunk:
             del work   # the caching allocator keeps it for the stream until the kernels have run
         return DeviceChunk(out, voxel_offset=self.voxel_offset, voxel_size=self.voxel_size, layer_type=self.layer_type)
 
+    def _ids(self, op: str):
+        """(contiguous (z, y, x) tensor, DTYPE_U32 / DTYPE_U64) of a segmentation of uint32 / int32 / uint64 / int64 ids."""
+        torch = _torch()
+        t = self.tensor.contiguous()
+        if t.ndim != 3:
+            raise ValueError(f"{op} takes a (z, y, x) segmentation, not a {t.ndim}-D chunk")
+        codes = {torch.int32: _native.DTYPE_U32, torch.int64: _native.DTYPE_U64}
+        for name, code in (("uint32", _native.DTYPE_U32), ("uint64", _native.DTYPE_U64)):
+            if hasattr(torch, name):
+                codes[getattr(torch, name)] = code
+        if t.dtype not in codes:
+            raise TypeError(f"{op} takes uint32, int32, uint64 or int64 ids, not {t.dtype}")
+        return t, codes[t.dtype]
+
+    def _physical_voxel_size(self, voxel_size) -> tuple:
+        vs = self.voxel_size if voxel_size is None else voxel_size
+        vs = tuple(float(v) for v in (vs if vs is not None else (1, 1, 1)))
+        if len(vs) != 3:
+            raise ValueError(f"the voxel size is (z, y, x), not {vs}")
+        return vs
+
     # ---- `mesh`: marching cubes on the device, welding and simplification on the host --------------------------------------
     def mesh(self, voxel_size=None, simplification_factor: int = 100, max_simplification_error: float = 40, skip_ids=None,
              close: bool = False, threads: int = 0) -> dict:
@@ -712,22 +734,10 @@ class DeviceChunk:
         pattern); another dtype raises TypeError and another ndim ValueError before any kernel runs.  The meshes are welded on
         the device; ``threads``: host workers of the simplifier (0: the hardware's); the result does not depend on it."""
         torch = _torch()
-        t = self.tensor.contiguous()
-        if t.ndim != 3:
-            raise ValueError(f"mesh takes a (z, y, x) segmentation, not a {t.ndim}-D chunk")
-        codes = {torch.int32: _native.DTYPE_U32, torch.int64: _native.DTYPE_U64}
-        for name, code in (("uint32", _native.DTYPE_U32), ("uint64", _native.DTYPE_U64)):
-            if hasattr(torch, name):
-                codes[getattr(torch, name)] = code
-        if t.dtype not in codes:
-            raise TypeError(f"mesh takes uint32, int32, uint64 or int64 ids, not {t.dtype}")
+        t, code = self._ids("mesh")
         if isinstance(simplification_factor, bool) or not isinstance(simplification_factor, (int, np.integer)):
             raise TypeError("the simplification factor is an integer")
-        vs = self.voxel_size if voxel_size is None else voxel_size
-        vs = tuple(float(v) for v in (vs if vs is not None else (1, 1, 1)))
-        if len(vs) != 3:
-            raise ValueError(f"the voxel size is (z, y, x), not {vs}")
-        code = codes[t.dtype]
+        vs = self._physical_voxel_size(voxel_size)
         skip = selected_ids(skip_ids) if skip_ids is not None else np.zeros(0, np.uint64)
         skip = np.unique(skip)
         zyx = tuple(t.shape)
@@ -752,6 +762,52 @@ class DeviceChunk:
         with ThreadPoolExecutor(max_workers=workers) as pool:
             out = pool.map(lambda k: _native.mesh_simplify_host(*meshes[k], simplification_factor, max_simplification_error), keys)
             return dict(zip(keys, out))
+
+    # ---- `skeletonize`: distance transform, geodesic field and TEASAR rounds on the device -----------------------------------
+    def distance_transform(self, voxel_size=None) -> "DeviceChunk":
+        """float32 distance of every voxel of a (z, y, x) segmentation to the nearest voxel of another id, outside the chunk
+        counting as 0 (0 for id 0), in physical units (csrc/skeleton.cu; for integer voxel sizes bit-identical to
+        scipy.ndimage.distance_transform_edt of each label's padded mask).  ``voxel_size`` is (z, y, x), the chunk's by default."""
+        torch = _torch()
+        t, code = self._ids("distance_transform")
+        vs = self._physical_voxel_size(voxel_size)
+        out = torch.empty(t.shape, dtype=torch.float32, device=t.device)
+        with self._on_device():
+            work = torch.empty(_native.edt_workspace(tuple(t.shape)), dtype=torch.uint8, device=t.device)
+            _native.edt_device(t.data_ptr(), code, tuple(t.shape), vs, out.data_ptr(), work.data_ptr(), self._stream())
+            del work
+        return DeviceChunk(out, voxel_offset=self.voxel_offset, voxel_size=self.voxel_size)
+
+    def skeletonize(self, voxel_size=None, scale: float = 4, const: float = 500, pdrf_scale: float = 100000, pdrf_exponent: int = 4,
+                    dust_threshold: int = 1000, skip_ids=None, stats: Optional[dict] = None) -> dict:
+        """TEASAR skeletons of every object of a (z, y, x) segmentation (csrc/skeleton.cu, rules in
+        oracle/skeleton_oracle.py; not kimimaro's skeletons): ``{id: Skeleton}`` in the chunk's own frame (vertices at voxel
+        centres, x, y, z in physical units), ids ascending.  An object is a 26-connected component of one id; 0, the
+        ``skip_ids`` and components of fewer than ``dust_threshold`` voxels are not skeletonized.  Same dtype and ndim checks as
+        ``mesh``.  ``stats``, when given, receives the relaxation sweeps, rounds, paths and phase times of the call."""
+        from ..flow.skeleton import Skeleton, check_params
+        torch = _torch()
+        t, code = self._ids("skeletonize")
+        vs = self._physical_voxel_size(voxel_size)
+        check_params(scale, const, pdrf_scale, pdrf_exponent, dust_threshold, vs, tuple(t.shape))
+        skip = np.unique(selected_ids(skip_ids) if skip_ids is not None else np.zeros(0, np.uint64))
+        zyx = tuple(t.shape)
+        if min(zyx) == 0:
+            return {}
+        with self._on_device():
+            d_skip = torch.from_numpy(skip.view(np.int64)).to(t.device) if skip.size else None
+            work = torch.empty(_native.skeleton_workspace(zyx), dtype=torch.uint8, device=t.device)
+            args = (t.data_ptr(), code, zyx, vs)
+            counts = _native.skeleton_count_device(*args, d_skip.data_ptr() if d_skip is not None else 0, skip.size, int(dust_threshold),
+                                                   work.data_ptr(), self._stream())
+            buf = torch.empty(max(counts[2], 1), dtype=torch.uint8, device=t.device)
+            n, st = _native.skeleton_device(*args, float(scale), float(const), float(pdrf_scale), int(pdrf_exponent), work.data_ptr(), counts,
+                                            buf.data_ptr(), self._stream())
+            out = _native.skeleton_read(buf.data_ptr(), zyx, vs, counts, n, self._stream())
+            del buf, work
+        if stats is not None:
+            stats.update(st)
+        return {k: Skeleton(*v) for k, v in out.items()}
 
     def __repr__(self):
         return f"DeviceChunk(shape={self.shape}, dtype={self.dtype}, voxel_offset={tuple(self.voxel_offset)}, device={self.tensor.device})"

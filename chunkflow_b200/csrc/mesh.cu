@@ -26,6 +26,7 @@ constexpr int kMcThreads = 256;
 
 #include "mesh_kernels.cuh"
 #include "raster_scan.cuh"
+#include "radix_sort.cuh"
 
 McGrid mc_grid(int64_t z, int64_t y, int64_t x, int32_t close) {
   if (z <= 0 || y <= 0 || x <= 0 || z > INT32_MAX || y > INT32_MAX || x > INT32_MAX) throw std::invalid_argument("mesh: bad volume size");
@@ -40,8 +41,6 @@ McGrid mc_grid(int64_t z, int64_t y, int64_t x, int32_t close) {
 }
 
 int64_t mc_blocks(int64_t items) { return ceil_div64(items, kMcBlock); }
-int64_t mc_chunks(int64_t items) { return ceil_div64(items, kMcChunk); }
-int mc_grid_size(int64_t work) { return (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div64(work, kMcThreads), 132 * 8)); }
 
 void mc_check(const void* d_labels, int32_t dtype, const void* d_skip, int64_t num_skip, const void* d_workspace) {
   if (!d_labels || !d_workspace) throw std::invalid_argument("mesh: null argument");
@@ -105,32 +104,6 @@ McBuffer mc_buffer(void* base, int64_t P, int64_t V, int64_t T) {
   u += 3 * V;
   b.bytes = (int64_t)((char*)u - (char*)base);
   return b;
-}
-
-// exclusive scan of n uint32 in place -> the total
-uint32_t mc_scan(uint32_t* a, int64_t n, uint32_t* sums, cudaStream_t s) {
-  const int64_t chunks = mc_chunks(n);
-  launch(mc_chunk_sum_kernel, mc_grid_size(chunks), kMcThreads, 0, s, a, n, sums);
-  launch(cc_scan_blocks_kernel, 1, 1024, 0, s, sums, chunks, sums + chunks);
-  launch(mc_chunk_scan_kernel, mc_grid_size(chunks), kMcThreads, 0, s, a, n, (const uint32_t*)sums);
-  uint32_t total = 0;
-  CFB_CUDA(cudaMemcpyAsync(&total, sums + chunks, 4, cudaMemcpyDeviceToHost, s));
-  CFB_CUDA(cudaStreamSynchronize(s));
-  return total;
-}
-
-// stable sort of (ids, vals) by the low `bits` bits of the ids; the result is back in ids, vals (an even number of passes)
-void mc_sort(unsigned long long* ids, unsigned long long* vals, unsigned long long* ids2, unsigned long long* vals2, int64_t n, int bits,
-             uint32_t* hist, uint32_t* sums, cudaStream_t s) {
-  const int64_t chunks = mc_chunks(n);
-  for (int shift = 0; shift < bits; shift += 8) {
-    launch(mc_radix_hist_kernel, mc_grid_size(chunks), kMcThreads, 0, s, (const unsigned long long*)ids, n, shift, hist);
-    mc_scan(hist, 256 * chunks, sums, s);
-    launch(mc_radix_scatter_kernel, mc_grid_size(chunks), kMcThreads, 0, s, (const unsigned long long*)ids,
-           (const unsigned long long*)vals, n, shift, (const uint32_t*)hist, ids2, vals2);
-    std::swap(ids, ids2);
-    std::swap(vals, vals2);
-  }
 }
 
 // runs of equal ids of a sorted stream: flag, rank (object of every item), start of every object -> objects

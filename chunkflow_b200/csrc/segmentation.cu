@@ -53,27 +53,6 @@ __global__ void __launch_bounds__(kT) cc_init_kernel(const T* __restrict__ in, u
   }
 }
 
-// backward half of the 26-neighbourhood, ordered so that the first 3 are the face neighbours (6-connectivity), the first 9
-// the face + edge neighbours (18) and all 13 the full neighbourhood (26)
-__constant__ int kNb[13][3] = {{0, 0, -1}, {0, -1, 0}, {-1, 0, 0},
-                               {0, -1, -1}, {0, -1, 1}, {-1, 0, -1}, {-1, 0, 1}, {-1, -1, 0}, {-1, 1, 0},
-                               {-1, -1, -1}, {-1, -1, 1}, {-1, 1, -1}, {-1, 1, 1}};
-
-__global__ void __launch_bounds__(kT) cc_merge_kernel(const uint32_t* __restrict__ val, uint32_t* __restrict__ P, Int3 sz, int nnb) {
-  const int64_t n = (int64_t)sz.z * sz.y * sz.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    const uint32_t v = val[i];
-    if (!v) continue;
-    const int x = (int)(i % sz.x), y = (int)((i / sz.x) % sz.y), z = (int)(i / ((int64_t)sz.x * sz.y));
-    for (int k = 0; k < nnb; ++k) {
-      const int zz = z + kNb[k][0], yy = y + kNb[k][1], xx = x + kNb[k][2];
-      if (zz < 0 || yy < 0 || yy >= sz.y || xx < 0 || xx >= sz.x) continue;
-      const int64_t j = ((int64_t)zz * sz.y + yy) * sz.x + xx;
-      if (val[j] == v) uf_unite(P, (uint32_t)i, (uint32_t)j);
-    }
-  }
-}
-
 // flatten + per-block count of roots
 __global__ void __launch_bounds__(kT) cc_flatten_count_kernel(const uint32_t* __restrict__ val, uint32_t* __restrict__ P, int64_t n,
                                                               uint32_t* __restrict__ block_count) {
@@ -171,7 +150,7 @@ extern "C" int cfb_connected_components_device(const void* d_in, int32_t in_dtyp
     else if (in_dtype == CFB_DTYPE_U32) launch(cc_init_kernel<uint32_t>, grid_for(n), kT, 0, s, (const uint32_t*)d_in, P, val, n, 0.f);
     else if (in_dtype == CFB_DTYPE_F32) launch(cc_init_kernel<float>, grid_for(n), kT, 0, s, (const float*)d_in, P, val, n, threshold);
     else throw std::invalid_argument("connected components: input dtype must be uint8, uint32 or float32 (with a threshold)");
-    launch(cc_merge_kernel, grid_for(n), kT, 0, s, val, P, sz, nnb);
+    launch(cc_merge_kernel<uint32_t>, grid_for(n), kT, 0, s, val, P, sz, nnb);
     launch(cc_flatten_count_kernel, (unsigned)nblocks, kT, 0, s, val, P, n, block_count);
     launch(cc_scan_blocks_kernel, 1, 1024, 0, s, block_count, nblocks, d_num);
     launch(cc_rank_kernel, (unsigned)nblocks, kT, 0, s, val, P, n, block_count, rank);

@@ -1,33 +1,10 @@
-// Device code of the `agglomerate` operator's voxel passes and the union-find helpers they share with connected components.
+// Device code of the `agglomerate` operator's voxel passes (the union-find they share with connected components: union_find.cuh).
 // NOT a stand-alone header: segmentation.cu includes it inside the library's anonymous namespace (after `Int3` and `kT`);
 // tests/host_emulation/ws_emulation.cpp compiles segmentation.cu for the host behind a one-thread CUDA shim, so that the
 // kernels and their launch sequences are checked against oracle/agglomeration_oracle.py on machines without a GPU as well.
 #pragma once
 
-__device__ __forceinline__ uint32_t uf_find(const uint32_t* P, uint32_t x) {
-  uint32_t p = P[x];
-  while (p != x) { x = p; p = P[x]; }
-  return x;
-}
-
-__device__ __forceinline__ void uf_unite(uint32_t* P, uint32_t a, uint32_t b) {
-  bool done = false;
-  do {
-    a = uf_find(P, a);
-    b = uf_find(P, b);
-    if (a < b) {
-      const uint32_t old = atomicMin(&P[b], a);
-      done = old == b;
-      b = old;
-    } else if (b < a) {
-      const uint32_t old = atomicMin(&P[a], b);
-      done = old == a;
-      a = old;
-    } else {
-      done = true;
-    }
-  } while (!done);
-}
+#include "union_find.cuh"
 
 
 // ------------------------------------------------------------------------------------------

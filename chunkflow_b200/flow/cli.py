@@ -506,5 +506,64 @@ def mesh(tasks, name, input_chunk_name, mip, voxel_size, output_path, output_for
         yield task
 
 
+@main.command("skeletonize")
+@click.option("--name", type=str, default="skeletonize", help="name of operator")
+@click.option("--input-chunk-name", "-i", type=str, default="chunk", help="name of the segmentation chunk to skeletonize.")
+@click.option("--voxel-size", "-v", type=click.FLOAT, nargs=3, default=None, callback=default_none,
+              help="voxel size of the segmentation, zyx order (default: the chunk's).")
+@click.option("--output-path", "-o", type=str, default="file:///tmp/skeleton/",
+              help="output path of the skeleton fragments: a local directory or file:// URL.")
+@click.option("--output-format", "-t", type=click.Choice(["precomputed", "swc"]), default="precomputed", help="fragment format.")
+@click.option("--scale", type=click.FLOAT, default=4, help="invalidation radius: scale * distance to boundary + const.")
+@click.option("--const", type=click.FLOAT, default=500, help="invalidation radius: scale * distance to boundary + const (nm).")
+@click.option("--pdrf-scale", type=click.FLOAT, default=100000, help="penalty field scale.")
+@click.option("--pdrf-exponent", type=click.INT, default=4, help="penalty field exponent (1 to 16).")
+@click.option("--dust-threshold", type=click.INT, default=1000, help="components with fewer voxels are not skeletonized.")
+@click.option("--skip-ids", "-s", type=str, default=None, help="ids not to skeletonize, separated by commas.")
+@operator
+def skeletonize(tasks, name, input_chunk_name, voxel_size, output_path, output_format, scale, const, pdrf_scale, pdrf_exponent,
+                dust_threshold, skip_ids):
+    """(extension) TEASAR skeletons of every object of a segmentation chunk on the GPU, written as ``{id}:{bbox}`` fragments
+    (reference plugins/skeletonize.py -> kimimaro; rules restated in oracle/skeleton_oracle.py, not kimimaro's skeletons).  A
+    host chunk is uploaded for the call, a GPU-resident one is skeletonized where it is."""
+    from chunkflow_b200.flow.skeleton import write_fragments
+    if skip_ids is not None:
+        skip_ids = sorted(set(map(int, skip_ids.split(","))))
+    for task in tasks:
+        if task is not None:
+            start = time()
+            seg = task[input_chunk_name]
+            dev, _ = _on_device(seg, "cuda:0")
+            vs = voxel_size if voxel_size is not None else tuple(seg.voxel_size)
+            skels = dev.skeletonize(voxel_size=vs, scale=scale, const=const, pdrf_scale=pdrf_scale, pdrf_exponent=pdrf_exponent,
+                                    dust_threshold=dust_threshold, skip_ids=skip_ids)
+            write_fragments(skels, output_path, tuple(seg.voxel_offset), seg.shape[-3:], vs, output_format)
+            task["log"]["timer"][name] = time() - start
+        yield task
+
+
+@main.command("aggregate-skeleton-fragments")
+@click.option("--name", type=str, default="aggregate-skeleton-fragments", help="name of operator")
+@click.option("--input-name", "-i", type=str, default="prefix", help="input prefix name in task stream.")
+@click.option("--prefix", "-p", type=str, default=None, help="prefix of skeleton fragments.")
+@click.option("--fragments-path", "-f", type=str, required=True, help="storage path of skeleton fragments.")
+@click.option("--output-path", "-o", type=str, default=None, help="storage path of aggregated skeletons.")
+@operator
+def aggregate_skeleton_fragments(tasks, name, input_name, prefix, fragments_path, output_path):
+    """Merge skeleton fragments (reference flow/flow.py:623-650): the fragments of every id are concatenated, equal vertices
+    merged and duplicate edges dropped.  kimimaro.postprocess (dust and tick removal, joining) is not applied."""
+    from chunkflow_b200.flow.skeleton import aggregate_fragments
+    if output_path is None:
+        output_path = fragments_path
+    if prefix:
+        aggregate_fragments(fragments_path, output_path, prefix)
+    for task in tasks:
+        if task is not None and not prefix:
+            start = time()
+            aggregate_fragments(fragments_path, output_path, task[input_name])
+            task["log"]["timer"][name] = time() - start
+        yield task
+
+
 if __name__ == "__main__":
     main()

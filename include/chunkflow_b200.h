@@ -608,6 +608,41 @@ int cfb_mesh_simplify_host(int64_t num_vertices, const float* vertices, int64_t 
                            int64_t simplification_factor, double max_simplification_error, int64_t* out_num_vertices,
                            float* out_vertices, int64_t* out_num_faces, uint32_t* out_faces);
 
+/* `skeletonize` (reference plugins/skeletonize.py -> kimimaro.skeletonize): a TEASAR skeleton of every object of a (z, y, x)
+ * segmentation, restated in oracle/skeleton_oracle.py (kimimaro is not vendored: its skeletons are not reproduced, parity
+ * unpinned).  dtype CFB_DTYPE_U32 or CFB_DTYPE_U64; voxel_size is (z, y, x), positive; the chunk has fewer than 2^32 voxels.
+ * Every error names the rule it broke in cfb_last_error.
+ * cfb_skeleton_workspace  bytes of d_workspace for a volume (about 30 bytes per voxel).  No device needed.
+ * cfb_edt_workspace  bytes of d_workspace for the distance transform alone (16 bytes per voxel).  No device needed.
+ * cfb_edt_device  d_dbf (float32, n) = the distance of every voxel to the nearest voxel of another id, outside the chunk being
+ *     0 (0 for id 0), in physical units.  d_workspace: cfb_edt_workspace bytes.
+ * cfb_skeleton_count_device  the distance transform and the objects (26-connected components of one non-zero id that is not
+ *     among the num_skip ascending d_skip_ids and has at least dust_threshold voxels) into d_workspace -> *num_objects, their
+ *     *num_voxels and the *buffer_bytes of d_buffer for cfb_skeleton_device (synchronises the stream).
+ * cfb_skeleton_device  after the count, with the same labels and workspace (one call per count: it overwrites the counts, and a
+ *     second call is refused): params = (scale, const, pdrf_scale), every one finite and >= 0, pdrf_exponent 1..16, and
+ *     (pdrf_scale + 1) * diagonal step * z * y * x * (1 + 2^-19) < 2^53 * the smallest voxel size, which keeps the geodesic
+ *     field finite and strictly increasing along every step.  -> *num_skeleton_voxels; stats (8 doubles, may be null) =
+ *     relaxation sweeps, rounds, paths, skeleton voxels, ms of the relaxation and parents, of the sort, of the rounds, and of the
+ *     trace kernels alone (host clock around work that ends in a synchronise).  Synchronises the stream.
+ * cfb_skeleton_read  the skeletons to the host, labels ascending (*num_labels <= num_objects entries of label_ids): label l has
+ *     the vertices vertex_offsets[l] .. vertex_offsets[l + 1] (rows of float32 x, y, z at voxel centres, and radii) and the edges
+ *     edge_offsets[l] .. edge_offsets[l + 1] (rows of two uint32 indices into its own vertices, sorted).  vertices and radii
+ *     have num_skeleton_voxels rows, edges num_skeleton_voxels - num_objects; the offsets num_objects + 1 entries. */
+int cfb_skeleton_workspace(int64_t z, int64_t y, int64_t x, int64_t* workspace_bytes);
+int cfb_edt_workspace(int64_t z, int64_t y, int64_t x, int64_t* workspace_bytes);
+int cfb_edt_device(const void* d_labels, int32_t dtype, int64_t z, int64_t y, int64_t x, const double* voxel_size, float* d_dbf,
+                   void* d_workspace, void* stream);
+int cfb_skeleton_count_device(const void* d_labels, int32_t dtype, int64_t z, int64_t y, int64_t x, const double* voxel_size,
+                              const uint64_t* d_skip_ids, int64_t num_skip, int64_t dust_threshold, void* d_workspace, int64_t* num_objects,
+                              int64_t* num_voxels, int64_t* buffer_bytes, void* stream);
+int cfb_skeleton_device(const void* d_labels, int32_t dtype, int64_t z, int64_t y, int64_t x, const double* voxel_size, const double* params,
+                        int32_t pdrf_exponent, void* d_workspace, int64_t num_objects, int64_t num_voxels, void* d_buffer,
+                        int64_t buffer_bytes, int64_t* num_skeleton_voxels, double* stats, void* stream);
+int cfb_skeleton_read(void* d_buffer, int64_t z, int64_t y, int64_t x, const double* voxel_size, int64_t num_objects, int64_t num_voxels,
+                      int64_t num_skeleton_voxels, int64_t* num_labels, uint64_t* label_ids, int64_t* vertex_offsets, int64_t* edge_offsets,
+                      float* vertices, uint32_t* edges, float* radii, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
