@@ -42,6 +42,8 @@ EXPORTS = (
     "cfb_clahe_workspace", "cfb_clahe_device",
     "cfb_mesh_workspace", "cfb_mesh_count_device", "cfb_mesh_buffer_bytes", "cfb_mesh_device", "cfb_mesh_read", "cfb_mesh_simplify_host",
     "cfb_skeleton_workspace", "cfb_edt_workspace", "cfb_edt_device", "cfb_skeleton_count_device", "cfb_skeleton_device", "cfb_skeleton_read",
+    "cfb_fill_holes_workspace", "cfb_fill_holes_table_workspace", "cfb_fill_holes_components_device", "cfb_fill_holes_graph_device",
+    "cfb_fill_holes_enclose", "cfb_fill_holes_apply_device",
 )
 
 
@@ -194,6 +196,7 @@ def load() -> C.CDLL:
     lib.cfb_clahe_device.argtypes = [vp, vp, i64, i64, i64, C.c_double, i32, i32, vp, i64, vp]
     bind_mesh(lib)
     bind_skeleton(lib)
+    bind_fill_holes(lib)
     for name in EXPORTS:
         getattr(lib, name)   # every declared symbol must be there
     _lib = lib
@@ -792,6 +795,72 @@ def skeleton_read(d_buffer: int, zyx, voxel_size, counts, num_skeleton_voxels: i
     _mesh_check(lib, lib.cfb_skeleton_read(C.c_void_p(d_buffer or None), *(int(v) for v in zyx), _ptr(vs), K, m, S, C.byref(nl), _ptr(ids),
                                            _ptr(vo), _ptr(eo), _ptr(verts), _ptr(edges), _ptr(radii), C.c_void_p(stream)))
     return {int(ids[i]): (verts[vo[i]:vo[i + 1]], edges[eo[i]:eo[i + 1]], radii[vo[i]:vo[i + 1]]) for i in range(int(nl.value))}
+
+
+# ---- `fill-segmentation-holes` (include/chunkflow_b200.h) ----
+FILL_MODES = ("binary", "keep-enclosed", "remove-enclosed")   # CFB_FILL_BINARY, CFB_FILL_KEEP_ENCLOSED, CFB_FILL_REMOVE_ENCLOSED
+
+
+def bind_fill_holes(lib: C.CDLL) -> None:
+    """Argument types of the fill-holes entry points (also for the host emulation of csrc/fill_holes.cu)."""
+    vp, i32, i64, pi64 = C.c_void_p, C.c_int32, C.c_int64, C.POINTER(C.c_int64)
+    lib.cfb_fill_holes_workspace.argtypes = [i64, i64, i64, pi64]
+    lib.cfb_fill_holes_table_workspace.argtypes = [i64, pi64]
+    lib.cfb_fill_holes_components_device.argtypes = [vp, i32, i64, i64, i64, i32, vp, pi64, vp]
+    lib.cfb_fill_holes_graph_device.argtypes = [vp, i64, i64, i64, vp, i64, pi64, vp]
+    lib.cfb_fill_holes_enclose.argtypes = [vp, i64, i64, i64, vp, i64, i64, vp]
+    lib.cfb_fill_holes_apply_device.argtypes = [vp, i32, i64, i64, i64, vp, vp, pi64, vp]
+
+
+def fill_mode(mode: str) -> int:
+    if mode not in FILL_MODES:
+        raise ValueError(f"fill holes: the mode is one of {FILL_MODES}, not {mode!r}")
+    return FILL_MODES.index(mode)
+
+
+def fill_holes_workspace(zyx, lib=None) -> int:
+    """Bytes of the per-voxel workspace of a (z, y, x) volume (no device needed)."""
+    lib, out = lib or load(), C.c_int64()
+    _mesh_check(lib, lib.cfb_fill_holes_workspace(*(int(v) for v in zyx), C.byref(out)))
+    return int(out.value)
+
+
+def fill_holes_table_workspace(table_slots: int, lib=None) -> int:
+    """Bytes of the pair table of ``table_slots`` slots (no device needed)."""
+    lib, out = lib or load(), C.c_int64()
+    _mesh_check(lib, lib.cfb_fill_holes_table_workspace(int(table_slots), C.byref(out)))
+    return int(out.value)
+
+
+def fill_holes_components_device(d_in: int, dtype: int, zyx, mode: str, d_workspace: int, stream: int = 0, lib=None) -> int:
+    """-> the number of components (of the background in binary mode, of every value otherwise); synchronises the stream."""
+    lib, n = lib or load(), C.c_int64()
+    _mesh_check(lib, lib.cfb_fill_holes_components_device(C.c_void_p(d_in), int(dtype), *(int(v) for v in zyx), fill_mode(mode),
+                                                          C.c_void_p(d_workspace), C.byref(n), C.c_void_p(stream)))
+    return int(n.value)
+
+
+def fill_holes_graph_device(d_workspace: int, zyx, d_table: int, table_slots: int, stream: int = 0, lib=None) -> int:
+    """-> the number of touching component pairs; raises NativeError with code ERR_CAPACITY when the table is too small."""
+    lib, n = lib or load(), C.c_int64()
+    _mesh_check(lib, lib.cfb_fill_holes_graph_device(C.c_void_p(d_workspace), *(int(v) for v in zyx), C.c_void_p(d_table), int(table_slots),
+                                                     C.byref(n), C.c_void_p(stream)))
+    return int(n.value)
+
+
+def fill_holes_enclose(d_workspace: int, zyx, d_table: int, table_slots: int, num_edges: int, stream: int = 0, lib=None) -> None:
+    """The encloser of every component, on the host (no GPU work but the copies)."""
+    lib = lib or load()
+    _mesh_check(lib, lib.cfb_fill_holes_enclose(C.c_void_p(d_workspace), *(int(v) for v in zyx), C.c_void_p(d_table), int(table_slots),
+                                                int(num_edges), C.c_void_p(stream)))
+
+
+def fill_holes_apply_device(d_in: int, dtype: int, zyx, d_workspace: int, d_out: int, stream: int = 0, lib=None) -> int:
+    """``d_out`` = the filled chunk -> the number of voxels the rule assigned; synchronises the stream."""
+    lib, n = lib or load(), C.c_int64()
+    _mesh_check(lib, lib.cfb_fill_holes_apply_device(C.c_void_p(d_in), int(dtype), *(int(v) for v in zyx), C.c_void_p(d_workspace),
+                                                     C.c_void_p(d_out), C.byref(n), C.c_void_p(stream)))
+    return int(n.value)
 
 
 def device_memory(device: int = 0) -> tuple:

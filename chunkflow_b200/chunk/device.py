@@ -19,6 +19,7 @@ bookkeeping of the reference's ``Chunk`` and mirrors, name for name, the referen
     clahe                reference plugins/clahe.py                     (plugin -> cv2.createCLAHE(...).apply)
     mesh                 reference flow/mesh.py                         (MeshOperator -> zmesh; rules restated)
     skeletonize          reference plugins/skeletonize.py               (plugin -> kimimaro; rules restated)
+    fill_holes           reference plugins/fill_segmentation_holes.py   (plugin -> fill_voids; rules restated)
 
 so that ``create-chunk | normalize-contrast | inference | crop-margin | quantize`` moves the image to the GPU once and
 brings a uint8 thumbnail (or nothing) back instead of the 12-byte-per-voxel affinity map.  There is no CPU fallback.
@@ -763,6 +764,65 @@ class DeviceChunk:
             out = pool.map(lambda k: _native.mesh_simplify_host(*meshes[k], simplification_factor, max_simplification_error), keys)
             return dict(zip(keys, out))
 
+    # ---- `fill-segmentation-holes`: components and their faces on the device, enclosure on the host ---------------------------
+    def fill_holes(self, mode: str = "binary", return_fill_count: bool = False, stats: Optional[dict] = None):
+        """fill_voids.fill of a (z, y, x) chunk and its per-object extensions (csrc/fill_holes.cu, rules in
+        oracle/fill_holes_oracle.py), 6-connected, outside = beyond the chunk's faces.  ``binary`` (the reference plugin): 1 for
+        every voxel != 0 and every background voxel with no background path to outside, 0 elsewhere; bool, uint8, int32, uint32,
+        int64, uint64 or float32.  ``keep-enclosed``: every 0 voxel enclosed by an object (a 6-connected component of one
+        non-zero id) takes the id of the innermost one.  ``remove-enclosed``: every enclosed voxel takes the id of the outermost
+        encloser.  The per-object modes take uint32 / int32 / uint64 / int64 ids (signed ones by their bit pattern).  Returns a
+        new chunk in the input's dtype (and, with ``return_fill_count``, the number of voxels the rule assigned: the holes, the
+        enclosed zeros, every enclosed voxel).  Another dtype, ndim or mode raises before any kernel runs.  ``stats``, when
+        given, receives the components, pairs, table slots and the ms of each phase (host clock around synchronised calls)."""
+        import time
+        torch = _torch()
+        code = _native.fill_mode(mode)
+        t = self.tensor.contiguous()
+        if t.ndim != 3:
+            raise ValueError(f"fill holes takes a (z, y, x) chunk, not a {t.ndim}-D one")
+        codes = {torch.bool: _native.DTYPE_U8, torch.uint8: _native.DTYPE_U8, torch.float32: _native.DTYPE_F32,
+                 torch.int32: _native.DTYPE_U32, torch.int64: _native.DTYPE_U64}
+        for name, c in (("uint32", _native.DTYPE_U32), ("uint64", _native.DTYPE_U64)):
+            if hasattr(torch, name):
+                codes[getattr(torch, name)] = c
+        if t.dtype not in codes or (code != 0 and codes[t.dtype] not in (_native.DTYPE_U32, _native.DTYPE_U64)):
+            allowed = "bool, uint8, int32, uint32, int64, uint64 or float32" if code == 0 else "uint32, int32, uint64 or int64 ids"
+            raise TypeError(f"fill holes: {mode} mode takes {allowed}, not {t.dtype}")
+        dtype, zyx = codes[t.dtype], tuple(t.shape)
+        out = torch.empty_like(t)
+        st = {"components": 0, "edges": 0, "table_slots": 0}
+        count = 0
+        if min(zyx) > 0:
+            with self._on_device():
+                s = self._stream()
+                t0 = time.perf_counter()
+                work = torch.empty(_native.fill_holes_workspace(zyx), dtype=torch.uint8, device=t.device)
+                st["components"] = comps = _native.fill_holes_components_device(t.data_ptr(), dtype, zyx, mode, work.data_ptr(), s)
+                t1 = time.perf_counter()
+                st["components_ms"] = (t1 - t0) * 1e3
+                if mode != "binary":
+                    slots = 1 << 16
+                    while slots < 4 * comps and slots < 1 << 30:
+                        slots <<= 1
+                    table, slots, edges = _grown_table(
+                        t.device, slots, _native.fill_holes_table_workspace,
+                        lambda table, slots: _native.fill_holes_graph_device(work.data_ptr(), zyx, table.data_ptr(), slots, s),
+                        "fill holes: more touching component pairs (at most 2^30)")
+                    t2 = time.perf_counter()
+                    _native.fill_holes_enclose(work.data_ptr(), zyx, table.data_ptr(), slots, edges, s)
+                    del table
+                    t3 = time.perf_counter()
+                    st.update(edges=edges, table_slots=slots, graph_ms=(t2 - t1) * 1e3, enclose_ms=(t3 - t2) * 1e3)
+                    t1 = t3
+                count = _native.fill_holes_apply_device(t.data_ptr(), dtype, zyx, work.data_ptr(), out.data_ptr(), s)
+                st["apply_ms"] = (time.perf_counter() - t1) * 1e3
+                del work
+        if stats is not None:
+            stats.update(st)
+        res = DeviceChunk(out, voxel_offset=self.voxel_offset, voxel_size=self.voxel_size, layer_type=self.layer_type)
+        return (res, count) if return_fill_count else res
+
     # ---- `skeletonize`: distance transform, geodesic field and TEASAR rounds on the device -----------------------------------
     def distance_transform(self, voxel_size=None) -> "DeviceChunk":
         """float32 distance of every voxel of a (z, y, x) segmentation to the nearest voxel of another id, outside the chunk
@@ -779,14 +839,20 @@ class DeviceChunk:
         return DeviceChunk(out, voxel_offset=self.voxel_offset, voxel_size=self.voxel_size)
 
     def skeletonize(self, voxel_size=None, scale: float = 4, const: float = 500, pdrf_scale: float = 100000, pdrf_exponent: int = 4,
-                    dust_threshold: int = 1000, skip_ids=None, stats: Optional[dict] = None) -> dict:
+                    dust_threshold: int = 1000, skip_ids=None, stats: Optional[dict] = None, fill_holes: bool = False) -> dict:
         """TEASAR skeletons of every object of a (z, y, x) segmentation (csrc/skeleton.cu, rules in
         oracle/skeleton_oracle.py; not kimimaro's skeletons): ``{id: Skeleton}`` in the chunk's own frame (vertices at voxel
         centres, x, y, z in physical units), ids ascending.  An object is a 26-connected component of one id; 0, the
         ``skip_ids`` and components of fewer than ``dust_threshold`` voxels are not skeletonized.  Same dtype and ndim checks as
-        ``mesh``.  ``stats``, when given, receives the relaxation sweeps, rounds, paths and phase times of the call."""
+        ``mesh``.  ``stats``, when given, receives the relaxation sweeps, rounds, paths and phase times of the call.
+        ``fill_holes``: the objects are first filled with ``fill_holes("remove-enclosed")`` (kimimaro's fill_holes: labels that
+        get filled in are deleted), so that a cavity does not make the skeleton loop around it."""
         from ..flow.skeleton import Skeleton, check_params
         torch = _torch()
+        if fill_holes:
+            self._ids("skeletonize")
+            return self.fill_holes("remove-enclosed").skeletonize(voxel_size, scale, const, pdrf_scale, pdrf_exponent, dust_threshold,
+                                                                  skip_ids, stats)
         t, code = self._ids("skeletonize")
         vs = self._physical_voxel_size(voxel_size)
         check_params(scale, const, pdrf_scale, pdrf_exponent, dust_threshold, vs, tuple(t.shape))

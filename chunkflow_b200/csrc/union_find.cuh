@@ -1,6 +1,7 @@
 // Label-equivalence union-find over the voxels' linear indices (lock-free: a root search and an atomicMin on the larger root),
-// shared by `connected-components` and the watershed (segmentation.cu) and by `skeletonize` (skeleton.cu, 26-connected objects
-// of uint32 or uint64 ids).  The root of a set is its smallest index.
+// shared by `connected-components` and the watershed (segmentation.cu), by `skeletonize` (skeleton.cu, 26-connected objects
+// of uint32 or uint64 ids) and by `fill-segmentation-holes` (fill_holes.cu, 6-connected components of every value, 0
+// included, or of the background alone).  The root of a set is its smallest index.
 // NOT a stand-alone header: included inside the library's anonymous namespace (after `Int3`).
 #pragma once
 
@@ -35,12 +36,16 @@ __constant__ int kNb[13][3] = {{0, 0, -1}, {0, -1, 0}, {-1, 0, 0},
                                {0, -1, -1}, {0, -1, 1}, {-1, 0, -1}, {-1, 0, 1}, {-1, -1, 0}, {-1, 1, 0},
                                {-1, -1, -1}, {-1, -1, 1}, {-1, 1, -1}, {-1, 1, 1}};
 
-template <typename V>
+// which voxels join their equal neighbours: the non-zero ones, every one, or the zero ones (for float32, +0 and -0 are zero
+// and NaN is not)
+enum { kJoinNonZero = 0, kJoinAll = 1, kJoinZero = 2 };
+
+template <typename V, int kJoin = kJoinNonZero>
 __global__ void __launch_bounds__(256) cc_merge_kernel(const V* __restrict__ val, uint32_t* __restrict__ P, Int3 sz, int nnb) {
   const int64_t n = (int64_t)sz.z * sz.y * sz.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const V v = val[i];
-    if (!v) continue;
+    if (kJoin == kJoinNonZero ? !v : kJoin == kJoinZero ? !!v : false) continue;
     const int x = (int)(i % sz.x), y = (int)((i / sz.x) % sz.y), z = (int)(i / ((int64_t)sz.x * sz.y));
     for (int k = 0; k < nnb; ++k) {
       const int zz = z + kNb[k][0], yy = y + kNb[k][1], xx = x + kNb[k][2];

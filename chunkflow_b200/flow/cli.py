@@ -463,6 +463,30 @@ def remap_segmentation(tasks, input_chunk_name, output_chunk_name, base_id):
         yield task
 
 
+@main.command("fill-segmentation-holes")
+@click.option("--input-chunk-name", "-i", type=str, default="chunk", help="input chunk name")
+@click.option("--output-chunk-name", "-o", type=str, default="chunk", help="output chunk name")
+@click.option("--mode", type=click.Choice(["binary", "keep-enclosed", "remove-enclosed"]), default="binary",
+              help="binary: fill_voids.fill (1 for the foreground and its holes); keep-enclosed: every 0 voxel enclosed by an object "
+                   "takes the id of the innermost one; remove-enclosed: every enclosed voxel takes the id of the outermost encloser.")
+@operator
+def fill_segmentation_holes(tasks, input_chunk_name, output_chunk_name, mode):
+    """(extension) Fill the holes of a segmentation chunk on the GPU, 6-connected, outside being beyond the chunk's faces
+    (the reference runs it as `plugin -f fill_segmentation_holes`, plugins/fill_segmentation_holes.py -> fill_voids.fill; rules
+    restated in oracle/fill_holes_oracle.py).  A host chunk comes back to the host, a GPU-resident one stays there."""
+    import torch
+    for task in tasks:
+        if task is not None:
+            dev, was_host = _on_device(task[input_chunk_name], "cuda:0")
+            out = dev.fill_holes(mode)
+            torch.cuda.synchronize(out.tensor.device)
+            if was_host:
+                out = Chunk(out.to_chunk().array, voxel_offset=out.voxel_offset, voxel_size=out.voxel_size,
+                            layer_type=getattr(task[input_chunk_name], "_layer_type", None))
+            task[output_chunk_name] = out
+        yield task
+
+
 @main.command("mesh")
 @click.option("--name", type=str, default="mesh", help="name of operator")
 @click.option("--input-chunk-name", "-i", type=str, default="chunk", help="name of chunk needs to be meshed.")
@@ -520,9 +544,11 @@ def mesh(tasks, name, input_chunk_name, mip, voxel_size, output_path, output_for
 @click.option("--pdrf-exponent", type=click.INT, default=4, help="penalty field exponent (1 to 16).")
 @click.option("--dust-threshold", type=click.INT, default=1000, help="components with fewer voxels are not skeletonized.")
 @click.option("--skip-ids", "-s", type=str, default=None, help="ids not to skeletonize, separated by commas.")
+@click.option("--fill-holes/--no-fill-holes", default=False,
+              help="fill every object's holes first (fill-segmentation-holes --mode remove-enclosed).")
 @operator
 def skeletonize(tasks, name, input_chunk_name, voxel_size, output_path, output_format, scale, const, pdrf_scale, pdrf_exponent,
-                dust_threshold, skip_ids):
+                dust_threshold, skip_ids, fill_holes=False):
     """(extension) TEASAR skeletons of every object of a segmentation chunk on the GPU, written as ``{id}:{bbox}`` fragments
     (reference plugins/skeletonize.py -> kimimaro; rules restated in oracle/skeleton_oracle.py, not kimimaro's skeletons).  A
     host chunk is uploaded for the call, a GPU-resident one is skeletonized where it is."""
@@ -536,7 +562,7 @@ def skeletonize(tasks, name, input_chunk_name, voxel_size, output_path, output_f
             dev, _ = _on_device(seg, "cuda:0")
             vs = voxel_size if voxel_size is not None else tuple(seg.voxel_size)
             skels = dev.skeletonize(voxel_size=vs, scale=scale, const=const, pdrf_scale=pdrf_scale, pdrf_exponent=pdrf_exponent,
-                                    dust_threshold=dust_threshold, skip_ids=skip_ids)
+                                    dust_threshold=dust_threshold, skip_ids=skip_ids, fill_holes=fill_holes)
             write_fragments(skels, output_path, tuple(seg.voxel_offset), seg.shape[-3:], vs, output_format)
             task["log"]["timer"][name] = time() - start
         yield task

@@ -643,6 +643,45 @@ int cfb_skeleton_read(void* d_buffer, int64_t z, int64_t y, int64_t x, const dou
                       int64_t num_skeleton_voxels, int64_t* num_labels, uint64_t* label_ids, int64_t* vertex_offsets, int64_t* edge_offsets,
                       float* vertices, uint32_t* edges, float* radii, void* stream);
 
+/* `fill-segmentation-holes` (reference plugins/fill_segmentation_holes.py -> fill_voids.fill), rules restated in
+ * oracle/fill_holes_oracle.py (fill_voids is not vendored: its 0/1 output is restated, not pinned; the hole mask equals
+ * scipy.ndimage.binary_fill_holes(seg != 0)).  Connectivity 6 (face neighbours); "outside" is beyond the six faces of the
+ * (z, y, x) chunk, which has fewer than 2^32 voxels.  An object is a 6-connected component of one non-zero id; object O encloses
+ * voxel v (not in O) when every 6-connected path from v to outside passes through O.  The enclosers of a voxel are nested.
+ *   CFB_FILL_BINARY           foreground = value != 0 (float32: -0 is background, NaN foreground); a hole is a background voxel
+ *                             with no background path to outside.  Output 1 for foreground and holes, 0 elsewhere.  Count: the
+ *                             holes.  dtype CFB_DTYPE_U8 (bool, uint8), CFB_DTYPE_F32, CFB_DTYPE_U32, CFB_DTYPE_U64.
+ *   CFB_FILL_KEEP_ENCLOSED    every 0 voxel enclosed by an object takes the id of the innermost one; other voxels keep theirs.
+ *                             Count: the enclosed zeros.
+ *   CFB_FILL_REMOVE_ENCLOSED  every enclosed voxel, whatever its id, takes the id of the outermost encloser.  Count: every
+ *                             enclosed voxel.  The per-object modes take CFB_DTYPE_U32 or CFB_DTYPE_U64 (signed ids by their
+ *                             bit pattern).
+ * Any other mode or dtype returns CFB_ERR_INVALID_ARGUMENT before any kernel runs; every error names its rule.
+ * cfb_fill_holes_workspace        bytes of d_workspace (about 13 per voxel).  No device needed.
+ * cfb_fill_holes_table_workspace  bytes of d_table for table_slots, a power of two below 2^31.  No device needed.
+ * cfb_fill_holes_components_device  the 6-connected components (of the background in binary mode, of every value otherwise)
+ *     and which of them reach outside, into d_workspace -> *num_components.  Synchronises the stream.
+ * cfb_fill_holes_graph_device     (per-object modes) the distinct pairs of touching components into d_table -> *num_edges;
+ *     CFB_ERR_CAPACITY when the table is too full -- call again with more slots.  Synchronises the stream.
+ * cfb_fill_holes_enclose          (per-object modes) on the host: the innermost or outermost non-zero encloser of every component
+ *     (articulation points of the component graph with a virtual outside node, iterative Hopcroft-Tarjan), written into
+ *     d_workspace.  Synchronises the stream.
+ * cfb_fill_holes_apply_device     d_out (same dtype and size as d_in, not overlapping it) = the filled chunk -> *fill_count.  After
+ *     the components (binary) or the enclosure, with the same d_in.  Synchronises the stream. */
+#define CFB_FILL_BINARY 0
+#define CFB_FILL_KEEP_ENCLOSED 1
+#define CFB_FILL_REMOVE_ENCLOSED 2
+int cfb_fill_holes_workspace(int64_t z, int64_t y, int64_t x, int64_t* workspace_bytes);
+int cfb_fill_holes_table_workspace(int64_t table_slots, int64_t* table_bytes);
+int cfb_fill_holes_components_device(const void* d_in, int32_t dtype, int64_t z, int64_t y, int64_t x, int32_t mode, void* d_workspace,
+                                     int64_t* num_components, void* stream);
+int cfb_fill_holes_graph_device(void* d_workspace, int64_t z, int64_t y, int64_t x, void* d_table, int64_t table_slots, int64_t* num_edges,
+                                void* stream);
+int cfb_fill_holes_enclose(void* d_workspace, int64_t z, int64_t y, int64_t x, void* d_table, int64_t table_slots, int64_t num_edges,
+                           void* stream);
+int cfb_fill_holes_apply_device(const void* d_in, int32_t dtype, int64_t z, int64_t y, int64_t x, void* d_workspace, void* d_out,
+                                int64_t* fill_count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
